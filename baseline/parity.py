@@ -1,8 +1,10 @@
 """CHECKER ONLY -- token-id parity of this repo's CUDA engine against the UNMODIFIED reference on the SAME GPU.
 
-The north star asks for greedy ids "bit-exact" against the reference.  Both sides run bf16 on the B200 with the SAME
+The north star asks for greedy ids "bit-exact" against the reference.  Both sides run bf16 on the same GPU with the SAME
 weight tensors (the reference model's parameters are re-pointed at the HF model's storage): the reference through its
 own ``jacobi_greedy_search_multilevel`` (``lade/decoding.py:697-1259``), ours through ``LookaheadEngine.generate``.
+The reference's side can also come from a recording (``StoredReference``, written by tests/golden/gen_golden_parity.py),
+so that the comparison runs where the reference is not installed.
 
 What can and cannot be exact: random-init bf16 logits tie to within 0-3 bf16 ulps at a few positions of every run
 (SURVEY.md App. D.8), and the two sides cannot round identically everywhere -- the reference's ids themselves change
@@ -159,6 +161,38 @@ def _bf16_ulp(x: float, mant_bits: int = 7) -> float:
     return 2.0 ** (math.floor(math.log2(ax)) - mant_bits)
 
 
+class StoredReference:
+    """The reference's side of one parity run as recorded by tests/golden/gen_golden_parity.py: its ids, its
+    self-consistency report and, for every generated position, the top next-token logits of its model's teacher-forced
+    causal forward.  Stands in for the reference model in compare_ids(); a candidate outside the recorded top logits
+    counts as infinitely far below the top (never a tie)."""
+
+    def __init__(self, rec: dict, mant_bits: int):
+        self.rec = rec
+        self.ids = list(rec["ids"])
+        self.n_prompt = int(rec["n_prompt"])
+        self.steps = rec.get("steps")
+        self.mant_bits = mant_bits
+
+    def next_logits(self, i: int) -> dict:
+        """{token: logit} of the recorded top logits for position i (absolute index into the ids)."""
+        row = i - self.n_prompt
+        return dict(zip(self.rec["topk_ids"][row], self.rec["topk_logits"][row]))
+
+
+def _judge(ref_model, ref_ids: Sequence[int], i: int, ours_tok: int):
+    """(top logit, our candidate's logit, the reference's candidate's logit, top-2 margin, mantissa bits) at position i."""
+    if isinstance(ref_model, StoredReference):
+        lg = ref_model.next_logits(i)
+        top2 = sorted(lg.values(), reverse=True)[:2]
+        return (top2[0], lg.get(ours_tok, -float("inf")), lg.get(ref_ids[i], -float("inf")), top2[0] - top2[1],
+                ref_model.mant_bits)
+    logits = reference_next_logits(ref_model, ref_ids[:i])
+    srt = torch.topk(logits, 2).values
+    return (logits.max().item(), logits[ours_tok].item(), logits[ref_ids[i]].item(), (srt[0] - srt[1]).item(),
+            _mant_bits(ref_model))
+
+
 def compare_ids(our_generate: Callable[[List[int], int], List[int]], ref_ids: Sequence[int], n_prompt: int,
                 ref_model, tol_ulps: float = 3.0, max_divergences: int = 64, self_check: bool = True) -> dict:
     """Position-by-position comparison with forcing (see the module docstring).
@@ -168,7 +202,10 @@ def compare_ids(our_generate: Callable[[List[int], int], List[int]], ref_ids: Se
     the distance at which the reference disagrees with itself cannot be told apart from a tie."""
     ref_ids = list(ref_ids)
     total = len(ref_ids)
-    self_rep = reference_self_consistency(ref_model, ref_ids, n_prompt) if self_check and total - n_prompt >= 1 else None
+    self_rep = None
+    if self_check and total - n_prompt >= 1:
+        self_rep = ref_model.rec["self"] if isinstance(ref_model, StoredReference) else \
+            reference_self_consistency(ref_model, ref_ids, n_prompt)
     if self_rep is not None:
         tol_ulps = max(tol_ulps, self_rep["worst_below_top_ulps"])
     ours = list(our_generate(ref_ids[:n_prompt], total - n_prompt))
@@ -180,14 +217,11 @@ def compare_ids(our_generate: Callable[[List[int], int], List[int]], ref_ids: Se
         if i is None:
             length_ok = len(ours) == total
             break
-        logits = reference_next_logits(ref_model, ref_ids[:i])
-        top = logits.max().item()
-        ulp = _bf16_ulp(top, _mant_bits(ref_model))
-        la, lb = logits[ours[i]].item(), logits[ref_ids[i]].item()
-        srt = torch.topk(logits, 2).values
+        top, la, lb, margin, mant = _judge(ref_model, ref_ids, i, ours[i])
+        ulp = _bf16_ulp(top, mant)
         divergences.append({"index": i - n_prompt, "ours": int(ours[i]), "ref": int(ref_ids[i]),
                             "ours_below_top_ulps": round((top - la) / ulp, 2), "ref_below_top_ulps": round((top - lb) / ulp, 2),
-                            "ref_top2_margin_ulps": round((srt[0] - srt[1]).item() / ulp, 2)})
+                            "ref_top2_margin_ulps": round(margin / ulp, 2)})
         if len(divergences) >= max_divergences or i + 1 >= total:
             length_ok = True
             break

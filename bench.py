@@ -8,6 +8,7 @@ surface (lade.augment_all(); lade.config_lade(...); model.generate(...)) with th
 memory and the output read back to the host inside the timed region.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload 7b|13b|tiny]
+                  [--dump-outputs DIR]
 
 Extra objects on the JSON line: `roofline` (lookahead-attention kernel, HBM bound, timed live with CUDA
 events), `cpu_baseline` (the oracle port of the reference's loop on the host cores, bounded sample),
@@ -69,6 +70,9 @@ def parse():
                     help="skip timing the unmodified reference's CUDA-eager loop (needs baseline/_ref)")
     ap.add_argument("--cuda-profiler-range", action="store_true",
                     help="cudaProfilerStart/Stop around the timed region (use with ncu --profile-from-start off)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed generate() returned as DIR/<name>.npy "
+                         "(token_ids: prompt + new tokens, float64) so that two builds can be compared output for output")
     return ap.parse_args()
 
 
@@ -78,14 +82,13 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s; not measured)"
 
 
 class ClockSampler:
-    """SM clock / throttle reasons during the timed region (B200_PROFILING.md recipe), sampled IN-PROCESS through NVML
-    (nvidia_ml_py) every 0.25 s.  Round 1 spawned `nvidia-smi` every 200 ms; on the 8-GPU node each spawn enumerates
-    all boards and the end-to-end leg lost half its throughput there.  Falls back to the subprocess at 1 Hz when NVML
-    cannot be loaded."""
+    """SM clock / throttle reasons during the timed region, sampled IN-PROCESS through NVML (nvidia_ml_py) every 0.25 s:
+    spawning `nvidia-smi` that often enumerates every board of a multi-GPU node and slows the end-to-end leg.  Falls
+    back to the subprocess at 1 Hz when NVML cannot be loaded."""
 
     REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap",
                0x80: "hw_power_brake_slowdown"}
@@ -295,22 +298,19 @@ def attn_roofline(eng, shape, reps=5):
     bytes_alg = 2 * kv_len * Hkv * D * 2 + q_len * Hq * D * 2 + 2 * q_len * Hkv * D * 2 + q_len * Hq * D * 2
     peak, how = measured_peaks()
     achieved = bytes_alg / (us * 1e-6) / 1e9
-    traffic = None            # DRAM bytes per launch from the committed ncu capture closest to this shape
-    try:
-        with open(os.path.join(ROOT, "profiles", "attn_traffic.json")) as f:
-            caps = [c for c in json.load(f)["captures"] if c["q_len"] == q_len]
-        if caps:
-            best = min(caps, key=lambda c: abs(c["kv_len"] - kv_len))
-            if abs(best["kv_len"] - kv_len) <= 64:
-                traffic = best["dram_bytes"]
-    except Exception:
-        traffic = None
     return {"bound": "hbm", "kernel": "lade_attn_fwd", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
-            "frac": round(achieved / peak, 4), "traffic": traffic, "peak_source": how, "us_per_launch": round(us, 2),
+            "frac": round(achieved / peak, 4), "peak_source": how, "us_per_launch": round(us, 2),
             "us_per_launch_serialized": round(us_serial, 2), "frac_serialized": round(bytes_alg / (us_serial * 1e-6) / 1e9 / peak, 4),
             "launch_mode": "programmatic dependent launch as in the decode step (set-up overlaps the predecessor's tail); "
                            "'serialized' = the same loop with the attribute off",
             "alg_bytes_per_launch": bytes_alg, "kv_len": kv_len, "q_len": q_len, "launches_timed": reps * eng.L}
+
+
+def dump_outputs(out_dir, token_ids):
+    """The arrays the timed path hands its caller, as float64 .npy (token ids are exact below 2^53)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "token_ids.npy"), np.asarray(token_ids, dtype=np.float64))
 
 
 def usable_cores() -> int:
@@ -543,7 +543,7 @@ def main():
               "parallelism": "single" if world == 1 else
               f"lookahead parallelism x{world} (lade_distributed: window columns + guess n-grams sharded per rank, "
               f"one NCCL all-gather of a fixed int32 record per step; same W/G => total work fixed)",
-              "l2_policy": "inputs larger than L2 (weights 13 GB/step stream through; KV of 32 layers > 126 MB)"}
+              "l2_policy": "inputs larger than L2 (weights 13 GB/step stream through; KV of 32 layers > the 50 MB L2)"}
     metric = "tokens/sec (wall-clock) and accepted-tokens/step, Llama-2-7B W=15 N=5 G=15" if args.workload == "7b" else \
         f"tokens/sec (wall-clock) and accepted-tokens/step, {args.workload} W={W} N={N} G={G}"
 
@@ -639,6 +639,8 @@ def main():
             torch.cuda.profiler.stop()
         dev_ms = e0.elapsed_time(e1)
         launches = eng.launches - launches0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, out)
         # ---- end to end through the plugin surface: pinned host prompt -> generate() -> host ids
         for _ in range(2):                                     # the HF generate() path has its own first-call costs
             model.generate(prompt_host.to(dev), attention_mask=torch.ones(1, P, dtype=torch.long, device=dev),

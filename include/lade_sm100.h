@@ -1,5 +1,5 @@
 /*
- * lade_sm100.h -- C ABI of the B200-native lookahead/verification decoding step.
+ * lade_sm100.h -- C ABI of the H100-native lookahead/verification decoding step.
  *
  * Drop-in boundary for ONE hot path of hao-ai-lab/LookaheadDecoding ("lade"): the Jacobi lookahead +
  * n-gram verification step.  Every entry point names the reference interface it replaces
@@ -160,22 +160,22 @@ int lade_rope_append(void* stream, const void* qkv, const void* cos_tab, const v
  * rowmask unused); all step rows see the committed cache.  Replaces LlamaAttention.forward's attention core (modeling_llama.py:520-541), the
  * dense mask of j_make_causal_mask_multilevel (:115-207) and flash_attn_lade.flash_attn_func(...,
  * lookahead=[...]) (:705-713).  `scratch` holds split-KV partials: lade_attn_scratch_bytes().
- * head_dim 128: tcgen05/TMA kernel (impl 0 or 2) or the mma.sync kernel (impl 1); head_dim 64 (TinyLlama-style): the
+ * head_dim 128: wgmma/TMA kernel (impl 0 or 2) or the mma.sync kernel (impl 1); head_dim 64 (TinyLlama-style): the
  * mma.sync kernel (impl 0 or 1).  Other head dimensions: LADE_EUNSUPPORTED.
- * impl 3 (head_dim 128): the tcgen05 kernel's REFERENCE-ORDER variant -- the probabilities are normalised by the sum
+ * impl 3 (head_dim 128): the wgmma kernel's REFERENCE-ORDER variant -- the probabilities are normalised by the sum
  * of the whole row in fp32 and rounded to the model dtype afterwards, exactly the order of :530-541 (impl 2 is an online
  * softmax: it rounds exp(x - max) before the sum is known, which changes the last bit of about half of the outputs).
- * Every S tile of a KV split stays in tensor memory, so kv_bound must be a true bound of kv_len + q_len and at most
+ * Every K/V tile of a KV split stays in shared memory, so kv_bound must be a true bound of kv_len + q_len and at most
  * 384 * n_splits (n_splits <= 8): LADE_EUNSUPPORTED otherwise.  Slower; a parity mode. */
 int lade_attn_fwd(void* stream, const void* q, const void* k_cache, const void* v_cache, void* out,
                   const uint32_t* rowmask, int32_t mask_words, const int32_t* meta, void* scratch, int32_t q_pad,
                   int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, int32_t kv_capacity,
                   int32_t kv_bound /* host upper bound of kv_len + q_len */, int32_t n_splits,
-                  int32_t impl /* 0 = default (= 2), 1 = mma.sync path, 2 = tcgen05/TMA path, 3 = its reference-order variant */);
+                  int32_t impl /* 0 = default (= 2), 1 = mma.sync path, 2 = wgmma/TMA path, 3 = its reference-order variant */);
 /* Bytes of zero-initialised scratch `lade_attn_fwd` needs for a shape (impl 1 keeps split partials there; the
- * tcgen05 path merges inside the cluster and only needs the buffer to exist).  No reference counterpart. */
+ * wgmma path merges inside the cluster and only needs the buffer to exist).  No reference counterpart. */
 int64_t lade_attn_scratch_bytes(int32_t q_pad, int32_t n_heads, int32_t head_dim, int32_t n_splits);
-/* Profiling aid: when set (device buffer of 8 int64 per CTA, or NULL to disable) the tcgen05 kernel records
+/* Profiling aid: when set (device buffer of 16 int64 per CTA, or NULL to disable) the wgmma kernel records
  * clock64() at its phase boundaries (start, first K tile landed, first S ready, O final, partials written,
  * siblings arrived, merged, end). */
 int lade_debug_attn_timing(void* dev_buffer);
@@ -187,7 +187,7 @@ int lade_debug_attn_timing(void* dev_buffer);
 int lade_debug_attn_pdl(int32_t enable);
 
 /* Projection GEMM of the lookahead step: c[m][n] (row stride ldc) = a[m][k] . w[n][k]^T, bf16 in/out, fp32
- * accumulation on tcgen05 tensor cores; w is an nn.Linear weight ([out_features][in_features], row-major).
+ * accumulation on the tensor cores (wgmma); w is an nn.Linear weight ([out_features][in_features], row-major).
  * Replaces q/k/v_proj (modeling_llama.py:447-449), o_proj (:541), gate/up/down_proj (:378) and lm_head (:1608)
  * for step row counts m <= 128; `a_rows` >= m is the number of addressable rows of the `a` buffer (rows >= m
  * are read but never stored).  tile_n / split_k = 0 lets the library pick (one wave of CTAs over the SMs);
@@ -207,13 +207,13 @@ int lade_swiglu(void* stream, const void* gate_up, void* out, int32_t rows, int3
  * `n_ctas` one-warp CTAs).  No reference counterpart: the reference streams every projection weight from DRAM when its
  * F.linear runs (modeling_llama.py:447-449,:378,:541).  Here the host queues the prefetch of the NEXT projection's
  * weights on a side branch of the step graph, parallel to the attention / norm / RoPE kernels, whose phases leave
- * HBM idle; the projection then finds (part of) its weights in the 126 MB L2.  ptr 16-byte aligned. */
+ * HBM idle; the projection then finds (part of) its weights in the 50 MB L2.  ptr 16-byte aligned. */
 int lade_l2_prefetch(void* stream, const void* ptr, int64_t bytes, int32_t n_ctas, int32_t chunk_bytes);
 
 /* fp16 models (the dtype of the reference's README.md:159 / minimal.py:19; the BASELINE configs are bf16): the same
  * kernels instantiated on the element type -- every rounding point of the bf16 entry point of the same name without the
  * suffix happens in fp16 instead.  Arguments, layouts and error codes are those of the unsuffixed function.
- * lade_attn_fwd_f16 picks its kernel like lade_attn_fwd (tcgen05/TMA for head_dim 128, mma.sync for 64 or impl 1). */
+ * lade_attn_fwd_f16 picks its kernel like lade_attn_fwd (wgmma/TMA for head_dim 128, mma.sync for 64 or impl 1). */
 int lade_rmsnorm_f16(void* stream, const void* x, const void* delta, const void* weight, void* h_out, void* out,
                      int32_t rows, int32_t hidden, float eps);
 int lade_rmsnorm_gather_f16(void* stream, const void* x, const void* delta, const void* weight,

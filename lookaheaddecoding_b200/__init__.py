@@ -1,4 +1,4 @@
-"""lookaheaddecoding_b200 -- B200-native (sm_100a) lookahead/verification decoding step.
+"""lookaheaddecoding_b200 -- H100-native (sm_90a) lookahead/verification decoding step.
 
 Drop-in for the hot path of hao-ai-lab/LookaheadDecoding behind the reference's plugin surface
 (lade/__init__.py:1-5):  ``augment_all()``, ``config_lade(...)``, then plain ``model.generate(...)``.

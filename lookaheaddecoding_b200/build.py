@@ -1,4 +1,4 @@
-"""In-tree nvcc build of liblade_sm100.so (sm_100a only).
+"""In-tree nvcc build of liblade_sm100.so (sm_90a only: the H100; the library keeps its historical name).
 
 The shared library is a plain C-ABI (include/lade_sm100.h); no torch headers are involved, so the
 build is a single nvcc invocation that also works on a GPU-less box (cross-compile).
@@ -18,7 +18,7 @@ LIB_PATH = os.path.join(LIB_DIR, "liblade_sm100.so")
 STAMP = os.path.join(LIB_DIR, "liblade_sm100.stamp")
 SOURCES = ["state.cu", "sampling.cu", "layer_ops.cu", "attn_mma.cu", "attn_tc.cu", "attn_api.cu", "gemm_tc.cu", "lp_nccl.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC", "-ldl",
 ]
 

@@ -36,8 +36,8 @@ int lade_attn_fwd(void* stream, const void* q, const void* k_cache, const void* 
   if (rowmask && mask_words * 32 < q_pad) return LADE_EINVAL;   // rowmask may be NULL for prefill-only use
   if (q_pad < 1 || n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads != 0 || n_splits < 1 || kv_capacity < 1)
     return LADE_EINVAL;
-  // impl 0 = the library's choice: the Blackwell-native tcgen05/TMA kernel for head_dim 128, the mma.sync kernel for the
-  // other instantiated head dimension (64); impl 2 / 1 force one of them; impl 3 = the tcgen05 kernel's reference-order
+  // impl 0 = the library's choice: the Hopper-native wgmma/TMA kernel for head_dim 128, the mma.sync kernel for the
+  // other instantiated head dimension (64); impl 2 / 1 force one of them; impl 3 = the wgmma kernel's reference-order
   // variant (probabilities normalised before they are rounded, like modeling_llama.py:530-541; kv_bound must bound
   // kv_len + q_len and fit 384 * n_splits)
   if (impl == 3)
@@ -51,7 +51,7 @@ int lade_attn_fwd(void* stream, const void* q, const void* k_cache, const void* 
 }
 
 /* fp16 models: the same attention with every rounding point in fp16 (the reference runs the module in the model dtype).
- * Same choice of kernel as the bf16 entry point: tcgen05/TMA for head_dim 128 (impl 0 or 2), mma.sync otherwise. */
+ * Same choice of kernel as the bf16 entry point: wgmma/TMA for head_dim 128 (impl 0 or 2), mma.sync otherwise. */
 int lade_attn_fwd_f16(void* stream, const void* q, const void* k_cache, const void* v_cache, void* out,
                       const uint32_t* rowmask, int32_t mask_words, const int32_t* meta, void* scratch, int32_t q_pad,
                       int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, int32_t kv_capacity,

@@ -1,12 +1,12 @@
 // Lookahead attention, legacy tensor-core path (mma.sync m16n8k16, cp.async staging).
 //
 // This is the robust first implementation (impl=1): split-KV flash attention over the persistent
-// KV cache with the lookahead mask evaluated in registers.  The tcgen05/TMA implementation
+// KV cache with the lookahead mask evaluated in registers.  The wgmma/TMA implementation
 // (attn_tc.cu, impl=2) is validated against it.  Replaces the attention core of
 // LlamaAttention.forward (lade/models/modeling_llama.py:520-541) + the dense additive mask of
 // j_make_causal_mask_multilevel (:115-207).
 //
-// Head dimensions 128 (Llama-2/3, CodeLlama) and 64 (TinyLlama-style) are instantiated; the tcgen05 path is built for
+// Head dimensions 128 (Llama-2/3, CodeLlama) and 64 (TinyLlama-style) are instantiated; the wgmma path is built for
 // 128 only, so 64 always runs here.
 //
 // Rounding points follow the reference: scores = bf16(QK^T) ; bf16(scores * (1/sqrt(D))) (torch's

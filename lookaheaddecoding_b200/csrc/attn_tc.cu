@@ -1,20 +1,28 @@
-// Lookahead attention, Blackwell-native path (impl=2): TMA-staged K/V tiles, tcgen05.mma with TMEM
-// accumulators, four softmax threads per query row, split-KV across a thread-block cluster with an in-kernel merge.
+// Lookahead attention, Hopper-native path (impl=2): TMA-staged K/V tiles, wgmma with register accumulators, the
+// lookahead mask evaluated in registers, split-KV across a thread-block cluster with an in-kernel merge.
 //
-// Per CTA: one (head, 128-row query tile, KV split).  Warp roles (576 threads):
-//   warp 0       TMA producer   Q tile + a 3-deep (long launches) or 2-deep (short launches) ring of K/V tiles
-//                               (128 kv rows x 128 d, SWIZZLE_128B)
-//   warp 1       MMA issuer     S = Q K^T  (kind::f16, M=128 N=128 K=16 x8, both operands K-major)
-//                               O += P V   (A = P K-major from smem, B = V MN-major from smem), L += P 1 (row sums),
-//                               TMEM alloc
-//   warps 2..17  softmax        four threads per query row (TMEM lane), each owning 32 of the tile's 128 kv
-//                               columns: tcgen05.ld -> reference rounding -> lookahead mask bits in registers
-//                               -> exp2 -> P (model dtype, swizzled into the K tile's smem); lazy O rescale in TMEM
-// TMEM: S double buffer (2 x 128 cols) + O (128 cols) + L (16 cols).
+// Per CTA: one (head, 128-row query tile, KV split).  Warp roles (288 threads):
+//   warps 0..7   two consumer warpgroups, 64 query rows each:
+//                  S = Q K^T    (wgmma m64n128k16, Q and K from shared memory, both K-major)
+//                  reference rounding -> mask bits -> exp2 -> P (model dtype) in registers, row max / sum by quad
+//                  shuffles (the four threads of a quad hold one row)
+//                  O += P V     (wgmma m64n128k16, P from registers, V from shared memory, MN-major)
+//   warp 8       TMA producer: Q tile + a 3-deep ring of K/V tiles (128 kv rows x 128 d, SWIZZLE_128B); it also zeroes
+//                the stale cache rows past kv_len + q_len of the last V tile (0 * NaN must not reach the MMA)
 // Split merge: fp32 partial rows pushed from registers into the owner CTA's shared memory (st.shared::cluster).
 //
 // Numerics follow attn_mma.cu / the reference (lade/models/modeling_llama.py:520-541); the mask is the
 // same register predicate (common.cuh row_sees == modeling_llama.py:115-207).
+//
+// The reference-order variant (impl 3, REF = true) runs the same tiles and MMAs but rounds the probabilities the way
+// the reference does (modeling_llama.py:530-541): p = model_dtype( exp(x - max_row) / sum_row ) with the max and the
+// sum of the WHOLE row (all KV splits), normalised in fp32 BEFORE the rounding, then P.V with fp32 accumulation.  The
+// online-softmax kernel has to round exp(x - max_so_far) before it knows the sum, which changes the last bit of about
+// half of the outputs (DESIGN.md 6).  Knowing the whole row first means: every K/V tile of a split stays resident in
+// shared memory (3 stages, so at most 3 KV tiles per split), S is recomputed by the tensor cores in each of the three
+// passes (row max, row sum, P.V), and the splits of a head meet twice in the middle of the kernel (row maxima, then row
+// sums, through an L2-resident table and a cluster barrier each).  It is an opt-in parity mode (impl = 3,
+// `LookaheadEngine(attn_impl=3)`): slower, and bounded to kv_len + q_len <= 384 * n_splits.
 #include "tc_common.cuh"
 
 #include <cstdlib>
@@ -27,46 +35,92 @@ namespace lade {
 constexpr int TC_BM = 128;
 constexpr int TC_BN = 128;
 constexpr int TC_D = 128;
-constexpr int TC_MAX_STAGES = 3;   // shared memory is sized for 3 K/V stages; the 2-stage instantiation turns the third into merge slots
-constexpr int TC_SOFTMAX_THREADS = 512;            // 16 warps: 4 threads per query row
-constexpr int TC_THREADS = 64 + TC_SOFTMAX_THREADS;
-constexpr int TC_TILE_BYTES = 128 * 128 * 2;   // one [128 x 128] bf16 tile = two [128 x 64] swizzle blocks
+constexpr int TC_STAGES = 3;
+constexpr int TC_CONSUMER_THREADS = 256;          // two warpgroups of 64 query rows
+constexpr int TC_THREADS = TC_CONSUMER_THREADS + 32;
+constexpr int TC_TILE_BYTES = 128 * 128 * 2;   // one [128 x 128] 16-bit tile = two [128 x 64] swizzle blocks
 constexpr int TC_HALF_BYTES = TC_TILE_BYTES / 2;
-constexpr int TC_XCH_FLOATS = 512;   // 2 KB: row maxima (bf16 [2][4][128]) / row sums (fp32 [4][128]) of the 4 threads of a row
-constexpr int TC_SMEM_TILES = TC_TILE_BYTES * (1 + 2 * TC_MAX_STAGES);
-constexpr int TC_ONES_OFFSET = TC_SMEM_TILES + 256 + TC_XCH_FLOATS * 4;   // 512 B of 1.0: B operand of the row-sum MMA
-constexpr int TC_SMEM_BYTES = TC_ONES_OFFSET + 512;
+constexpr int TC_SMEM_TILES = TC_TILE_BYTES * (1 + 2 * TC_STAGES);
+constexpr int TC_SMEM_BYTES = TC_SMEM_TILES + 256 + 1024;   // tiles + mbarriers + slack to align the base to 1024 B
 constexpr float TC_LOG2E = 1.4426950408889634f;
-// DSMEM merge transport (merge_mode 1).  3 stages: slots alias the owner's dead K/V stages, (m, l) its dead Q tile (a
-// cluster barrier separates compute from the pushes).  2 stages: the third stage's 64 KB are DEDICATED slots
-// ((n - 1) * ceil(128 / n) * 528 B <= 60,192 for n <= 8, then (m, l)), so a split pushes the moment it is done.
-constexpr int TC_SO_STRIDE = 132;                       // floats per staged O row (528 B: conflict-free float4 rows)
-constexpr int TC_SLOT_ML_OFFSET = 60416;                // (m, l) table inside the dedicated slot region
+// DSMEM merge: slots of [per][TC_SO_STRIDE] floats alias the owner's dead K/V stages, the (m, l) table its dead Q tile
+// (a cluster barrier separates compute from the pushes); (n - 1) * ceil(128 / n) * 528 B <= 59,136 for n <= 8.
+constexpr int TC_SO_STRIDE = 132;                       // floats per staged O row (528 B)
+constexpr int TC_SO_OFFSET = TC_TILE_BYTES;
+constexpr int TC_SML_OFFSET = 0;
 
-template <typename ET>
-__host__ __device__ constexpr uint32_t umma_idesc(bool b_mn_major) {
-  return umma_idesc_n(128u, b_mn_major, sizeof(ET) == 2 && !std::is_same<ET, __nv_bfloat16>::value);
-}
-
-// Optional per-CTA phase timestamps (clock64) for profiling the kernel's own timeline: 16 slots per CTA
-// (0-7 CTA phases, 8-15 the softmax phases of tile 1 as seen by thread 64).
+// Optional per-CTA phase timestamps (clock64) for profiling the kernel's own timeline: 16 slots per CTA, 0-7 used.
 __device__ long long* g_attn_timing = nullptr;
 #define TC_STAMP(slot, tid) do { if (tbuf && threadIdx.x == (tid)) tbuf[slot] = clock64(); } while (0)
 enum { TS_START = 0, TS_KFULL0 = 1, TS_SFULL0 = 2, TS_OFINAL = 3, TS_STAGED = 4, TS_CLUSTER = 5, TS_MERGED = 6, TS_END = 7 };
 
+// The model-dtype pair packed by Elem<ET>::pack2, back in fp32 (the rounded probabilities the row sum adds up).
+template <typename ET> __device__ __forceinline__ float2 unpack2(uint32_t u);
+template <> __device__ __forceinline__ float2 unpack2<__nv_bfloat16>(uint32_t u) {
+  return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));
+}
+template <> __device__ __forceinline__ float2 unpack2<__half>(uint32_t u) {
+  return __half22float2(*reinterpret_cast<__half2*>(&u));
+}
+
+// S[64 x 128] = Q[rows of warpgroup wg] . K^T of one stage.
+template <typename ET>
+__device__ __forceinline__ void qk_tile(float (&s)[64], uint32_t sQ_a, uint32_t sK_a, int wg) {
+  wg_fence();
+#pragma unroll
+  for (int kb = 0; kb < 2; ++kb)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t da = wg_desc(sQ_a + kb * TC_HALF_BYTES + wg * 8192 + k * 32, 16, 1024);
+      const uint64_t db = wg_desc(sK_a + kb * TC_HALF_BYTES + k * 32, 16, 1024);
+      wgmma_m64n128_ss<ET>(s, da, db, (kb | k) ? 1u : 0u);
+    }
+  wg_commit();
+  wg_wait_all();
+  wg_fence_regs(s);
+}
+
+// O[64 x 128] += P[64 x 128 kv] . V of one stage; p = the A fragments of the eight k16 steps (4 registers each).
+template <typename ET>
+__device__ __forceinline__ void pv_tile(float (&o)[64], const uint32_t (&p)[32], uint32_t sV_a) {
+  wg_fence_regs(o);
+  wg_fence();
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) wgmma_m64n128_rs_tb<ET>(o, p + 4 * kk, wg_desc(sV_a + kk * 2048, TC_HALF_BYTES, 1024));
+  wg_commit();
+  wg_wait_all();
+  wg_fence_regs(o);
+}
+
+// Visibility of the 32 columns a thread holds in each of its two rows: word w of row rr covers tile columns [32w, 32w+32).
+__device__ __forceinline__ void tile_mask(uint32_t (&mb)[2][4], const uint32_t* const (&mrow)[2], const int (&row)[2],
+                                          int mask_words, int tile0, int kv_len, int q_len, int is_prefill) {
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+    for (int w = 0; w < 4; ++w)
+      mb[rr][w] = (tile0 + 32 * w + 32 <= kv_len)
+                      ? 0xffffffffu
+                      : visible_bits32(mrow[rr], mask_words, tile0 + 32 * w, kv_len, q_len, is_prefill, row[rr]);
+}
+// accumulator element (i, e) of row half rr sits in tile column 8i + 2t + e: word i / 4, bit 8 (i % 4) + 2t + e
+__device__ __forceinline__ bool vis(const uint32_t (&mb)[2][4], int rr, int i, int e, int t) {
+  return (mb[rr][i >> 2] >> (8 * (i & 3) + 2 * t + e)) & 1u;
+}
 
 // ---- kernel ---------------------------------------------------------------------------------------------
-// grid (n_splits, heads, q tiles); when n_splits > 1 the n_splits CTAs of one (head, q tile) form a thread-block
-// cluster and merge their split-KV partials through distributed shared memory.
-template <typename ET, bool ROWSUM_MMA>
+// grid (n_splits, heads, q tiles); the n_splits CTAs of one (head, q tile) form a thread-block cluster and merge their
+// split-KV partials through distributed shared memory.
+template <typename ET, bool REF>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, ET* __restrict__ out,
                    const uint32_t* __restrict__ rowmask, int mask_words, const int* __restrict__ meta, int q_pad,
-                   int n_heads, int n_kv_heads, int n_splits, float inv_sqrt_d, float* __restrict__ part_o,
-                   float2* __restrict__ part_ml, int flags) {
-  constexpr bool rowsum_mma = ROWSUM_MMA;
-  extern __shared__ __align__(1024) unsigned char smem[];
+                   int n_heads, int n_kv_heads, int n_splits, float inv_sqrt_d, float2* __restrict__ row_ml) {
+  extern __shared__ unsigned char smem_raw[];
+  const uint32_t raw_a = smem_u32(smem_raw);
+  const uint32_t sQ_a = (raw_a + 1023u) & ~1023u;                  // SWIZZLE_128B tiles need 1024-byte alignment
+  unsigned char* smem = smem_raw + (sQ_a - raw_a);
   const int split = blockIdx.x, h = blockIdx.y, mt = blockIdx.z;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -84,773 +138,361 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   const bool active = split < n_active;
   const int tile_lo = split * t_base + (split < t_rem ? split : t_rem);
   const int my_tiles = active ? t_base + (split < t_rem ? 1 : 0) : 0;
+  if (REF && t_base + (t_rem ? 1 : 0) > TC_STAGES) __trap();     // the caller's kv_bound was not a bound (host checks it)
   const int hk = h / (n_heads / n_kv_heads);
   const int HD = n_heads * TC_D;
-  // K/V ring depth.  Short split-KV launches (no split holds more than (flags >> 8) tiles: the decode step at the
-  // benchmark's context) run a 2-deep ring and turn the third stage into DEDICATED merge slots: a split then pushes
-  // its partial the moment it is done -- the early finishers while the longest split still computes -- and the
-  // compute/push cluster barrier of the aliasing layout goes away.  Long launches keep 3 stages (the stream needs them).
-  const int merge_mode = flags & 1;
-  const int nst = (n_splits > 1 && merge_mode == 1 && t_base + (t_rem ? 1 : 0) <= ((flags >> 8) & 0xff)) ? 2 : 3;
-  const int TC_SO_OFFSET = nst == 2 ? TC_TILE_BYTES * 5 : TC_TILE_BYTES;
-  const int TC_SML_OFFSET = nst == 2 ? TC_TILE_BYTES * 5 + TC_SLOT_ML_OFFSET : 0;
+  const long long hm = (long long)h * gridDim.z + mt;
+  // a warpgroup whose 64 rows are all padding has nothing to compute
+  const int n_wg = (mt * TC_BM + 64 < q_pad) ? 2 : 1;
+  // the last tile of the launch may run past kv_len + q_len: its stale V rows are zeroed before P.V reads them
+  const bool zero_last = active && (tile_lo + my_tiles) * TC_BN > T;
   long long* tbuf = g_attn_timing ? g_attn_timing + 16ll * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
   TC_STAMP(TS_START, 0);
-  // programmatic dependent launch, producer side: a dependent grid (in the decode step: none -- the o_proj GEMM is a
-  // plain launch; in a back-to-back loop over layer caches: the next lookahead-attention launch) may be scheduled as
-  // soon as SMs free up; it orders itself with griddepcontrol.wait before it touches anything this grid writes
+  // programmatic dependent launch, producer side: a dependent grid may be scheduled as soon as SMs free up; it orders
+  // itself with griddepcontrol.wait before it touches anything this grid writes
   griddep_launch_dependents();
 
-  unsigned char* sQ = smem;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_SMEM_TILES);
-  // barrier slots: 0 q_full | 1.. k_full[S] | v_full[S] | stage_free[S] | s_full[2] | p_full[2] | o_final
+  // barrier slots: 0 q_full | 1.. k_full[S] | v_full[S] | stage_free[S] | v_zeroed
   const uint32_t bar0 = smem_u32(bars);
   auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  const int B_QFULL = 0, B_KFULL = 1, B_VFULL = 1 + TC_MAX_STAGES, B_FREE = 1 + 2 * TC_MAX_STAGES,
-            B_SFULL = 1 + 3 * TC_MAX_STAGES, B_PFULL = 3 + 3 * TC_MAX_STAGES, B_OFINAL = 5 + 3 * TC_MAX_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 24);
-  ET* s_xmax = reinterpret_cast<ET*>(smem + TC_SMEM_TILES + 256);   // [2][4][128] row maxima (model dtype: exact)
-  float* s_xsum = reinterpret_cast<float*>(smem + TC_SMEM_TILES + 256);                   // [4][128] row sums (epilogue)
-  const uint32_t sQ_a = smem_u32(sQ);
+  const int B_QFULL = 0, B_KFULL = 1, B_VFULL = 1 + TC_STAGES, B_FREE = 1 + 2 * TC_STAGES, B_VZERO = 1 + 3 * TC_STAGES;
   auto sK_a = [&](int s) { return sQ_a + (uint32_t)TC_TILE_BYTES * (1 + 2 * s); };
   auto sV_a = [&](int s) { return sQ_a + (uint32_t)TC_TILE_BYTES * (2 + 2 * s); };
+  auto issue_tile = [&](int j) {
+    const int s = j % TC_STAGES;
+    const int row0 = (tile_lo + j) * TC_BN;
+    mbar_expect_tx(BAR(B_KFULL + s), TC_TILE_BYTES);
+    tma_load_3d(sK_a(s), &tmK, BAR(B_KFULL + s), 0, row0, hk);
+    tma_load_3d(sK_a(s) + TC_HALF_BYTES, &tmK, BAR(B_KFULL + s), 64, row0, hk);
+    mbar_expect_tx(BAR(B_VFULL + s), TC_TILE_BYTES);
+    tma_load_3d(sV_a(s), &tmV, BAR(B_VFULL + s), 0, row0, hk);
+    tma_load_3d(sV_a(s) + TC_HALF_BYTES, &tmV, BAR(B_VFULL + s), 64, row0, hk);
+  };
 
-  if (active) {
-    if (threadIdx.x == 0) {
-      if ((sQ_a & 1023u) != 0) __trap();   // SWIZZLE_128B tiles need 1024-byte alignment
-      mbar_init(BAR(B_QFULL), 1);
-      for (int s = 0; s < TC_MAX_STAGES; ++s) { mbar_init(BAR(B_KFULL + s), 1); mbar_init(BAR(B_VFULL + s), 1); mbar_init(BAR(B_FREE + s), 1); }
-      for (int b = 0; b < 2; ++b) { mbar_init(BAR(B_SFULL + b), 1); mbar_init(BAR(B_PFULL + b), TC_SOFTMAX_THREADS / 32); }
-      mbar_init(BAR(B_OFINAL), 1);
-      fence_barrier_init();
-      // Start the memory stream before anything else, while the other warps allocate TMEM and meet at the barrier
-      // below.  With programmatic dependent launch this CTA may already be running while the producer of this
-      // step's Q and new K/V rows (lade_rope_append) is still in flight: cache tiles entirely below kv_len were
-      // written by earlier steps and are fetched at once; Q and tiles touching rows >= kv_len wait for the producer.
-      auto issue_tile = [&](int j) {
-        const int row0 = (tile_lo + j) * TC_BN;
-        mbar_expect_tx(BAR(B_KFULL + j), TC_TILE_BYTES);
-        tma_load_3d(sK_a(j), &tmK, BAR(B_KFULL + j), 0, row0, hk);
-        tma_load_3d(sK_a(j) + TC_HALF_BYTES, &tmK, BAR(B_KFULL + j), 64, row0, hk);
-        mbar_expect_tx(BAR(B_VFULL + j), TC_TILE_BYTES);
-        tma_load_3d(sV_a(j), &tmV, BAR(B_VFULL + j), 0, row0, hk);
-        tma_load_3d(sV_a(j) + TC_HALF_BYTES, &tmV, BAR(B_VFULL + j), 64, row0, hk);
-      };
-      const int n_pre = my_tiles < nst ? my_tiles : nst;
-      int n_old = 0;                                   // leading tiles that hold only rows of earlier steps
-      while (n_old < n_pre && (tile_lo + n_old + 1) * TC_BN <= kv_len) ++n_old;
-      for (int j = 0; j < n_old; ++j) issue_tile(j);
-      griddep_wait();
-      mbar_expect_tx(BAR(B_QFULL), TC_TILE_BYTES);
-      tma_load_3d(sQ_a, &tmQ, BAR(B_QFULL), 0, mt * TC_BM, h);
-      tma_load_3d(sQ_a + TC_HALF_BYTES, &tmQ, BAR(B_QFULL), 64, mt * TC_BM, h);
-      for (int j = n_old; j < n_pre; ++j) issue_tile(j);
+  if (active && threadIdx.x == TC_CONSUMER_THREADS) {
+    mbar_init(BAR(B_QFULL), 1);
+    for (int s = 0; s < TC_STAGES; ++s) {
+      mbar_init(BAR(B_KFULL + s), 1);
+      mbar_init(BAR(B_VFULL + s), 1);
+      mbar_init(BAR(B_FREE + s), 4 * n_wg);           // one arrival per consumer warp
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512);
-    if (rowsum_mma && threadIdx.x >= 64 && threadIdx.x < 64 + 128) {       // 256 x (1.0, 1.0) pairs of the model dtype
-      reinterpret_cast<uint32_t*>(smem + TC_ONES_OFFSET)[threadIdx.x - 64] = Elem<ET>::pack2(1.f, 1.f);
-      fence_proxy_async();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
+    mbar_init(BAR(B_VZERO), 1);
+    fence_barrier_init();
+    // Start the memory stream before anything else.  With programmatic dependent launch this CTA may already be
+    // running while the producer of this step's Q and new K/V rows (lade_rope_append) is still in flight: cache tiles
+    // entirely below kv_len were written by earlier steps and are fetched at once; Q and tiles touching rows >= kv_len
+    // wait for the producer.
+    const int n_pre = my_tiles < TC_STAGES ? my_tiles : TC_STAGES;
+    int n_old = 0;                                   // leading tiles that hold only rows of earlier steps
+    while (n_old < n_pre && (tile_lo + n_old + 1) * TC_BN <= kv_len) ++n_old;
+    for (int j = 0; j < n_old; ++j) issue_tile(j);
+    griddep_wait();
+    mbar_expect_tx(BAR(B_QFULL), TC_TILE_BYTES);
+    tma_load_3d(sQ_a, &tmQ, BAR(B_QFULL), 0, mt * TC_BM, h);
+    tma_load_3d(sQ_a + TC_HALF_BYTES, &tmQ, BAR(B_QFULL), 64, mt * TC_BM, h);
+    for (int j = n_old; j < n_pre; ++j) issue_tile(j);
   }
-  // 2-deep ring: the only thing a pusher must know about its target is that the CTA is resident (its slots are never
-  // used for anything else), so the cluster meets HERE, split-phase: arrive now, wait just before the first push
-  if (nst == 2) cluster_arrive();
-  const uint32_t tmem_base = active ? *tmem_slot : 0u;
-  const uint32_t tmem_O = tmem_base + 256;
-  const uint32_t tmem_L = tmem_base + 384;      // row sums by tensor core (rowsum_mma): 16 equal columns, column 0 is read
-  // a softmax thread's share of its split's result: 32 fp32 of the unnormalised O row + the row's (max, sum);
-  // they stay in registers across the role join for the split merge at the end of the kernel
-  float ov[32];
-  float m_row = -INFINITY, l_row = 0.f;
+  __syncthreads();
 
-  if (!active) {
-    // an idle split of the cluster: nothing to compute, but it must meet its siblings at the cluster barriers
-  } else if (warp == 0) {
-    // ================= TMA producer (tiles beyond the first STAGES; the rest was issued in the prologue) =====
-    if (lane == 0) {
-      for (int j = nst; j < my_tiles; ++j) {
-        const int s = j % nst;
-        mbar_wait(BAR(B_FREE + s), ((j / nst) - 1) & 1);
-        const int row0 = (tile_lo + j) * TC_BN;
-        mbar_expect_tx(BAR(B_KFULL + s), TC_TILE_BYTES);
-        tma_load_3d(sK_a(s), &tmK, BAR(B_KFULL + s), 0, row0, hk);
-        tma_load_3d(sK_a(s) + TC_HALF_BYTES, &tmK, BAR(B_KFULL + s), 64, row0, hk);
-        mbar_expect_tx(BAR(B_VFULL + s), TC_TILE_BYTES);
-        tma_load_3d(sV_a(s), &tmV, BAR(B_VFULL + s), 0, row0, hk);
-        tma_load_3d(sV_a(s) + TC_HALF_BYTES, &tmV, BAR(B_VFULL + s), 64, row0, hk);
-      }
-    }
-    __syncwarp();   // reconverge before the block-wide barrier below
-  } else if (warp == 1) {
-    // ================= MMA issuer (one thread) =================
-    if (lane == 0) {
-      constexpr uint32_t IDESC_QK = umma_idesc<ET>(false);
-      constexpr uint32_t IDESC_PV = umma_idesc<ET>(true);
-      auto issue_qk = [&](int j) {
-        const int s = j % nst;
-        mbar_wait(BAR(B_KFULL + s), (j / nst) & 1);
-        tc_fence_after();
-        const uint32_t d = tmem_base + (uint32_t)(j & 1) * 128u;
+  // a consumer thread's share of its split's result: two rows (g and g + 8 of its warp's 16) x 32 of the 128 columns,
+  // the unnormalised O (impl 2) or the normalised partial O (impl 3); kept in registers for the split merge
+  const int wg = warp >> 2;
+  const int g = lane >> 2, t = lane & 3;
+  const int rl[2] = {wg * 64 + (warp & 3) * 16 + g, wg * 64 + (warp & 3) * 16 + g + 8};   // rows inside the tile
+  const bool work = active && warp < 8 && wg < n_wg;
+  float o[64];
+  float m_row[2] = {-INFINITY, -INFINITY}, l_row[2] = {0.f, 0.f};
 #pragma unroll
-        for (int kb = 0; kb < 2; ++kb)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t da = umma_desc(sQ_a + kb * TC_HALF_BYTES + k * 32, 16, 1024);
-            const uint64_t db = umma_desc(sK_a(s) + kb * TC_HALF_BYTES + k * 32, 16, 1024);
-            umma_bf16(d, da, db, IDESC_QK, (kb | k) ? 1u : 0u);
-          }
-        umma_commit(BAR(B_SFULL + (j & 1)));
-      };
-      mbar_wait(BAR(B_QFULL), 0);
-      mbar_wait(BAR(B_KFULL), 0);
-      if (tbuf) tbuf[TS_KFULL0] = clock64();
-      issue_qk(0);
-      for (int j = 0; j < my_tiles; ++j) {
-        if (j + 1 < my_tiles) issue_qk(j + 1);
-        const int s = j % nst;
-        mbar_wait(BAR(B_PFULL + (j & 1)), (j >> 1) & 1);
-        mbar_wait(BAR(B_VFULL + s), (j / nst) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          // A = P tile (K-major, lives in the K stage), B = V tile (MN-major: LBO = next 64-wide d block)
-          const uint64_t da = umma_desc(sK_a(s) + (kk >> 2) * TC_HALF_BYTES + (kk & 3) * 32, 16, 1024);
-          const uint64_t db = umma_desc(sV_a(s) + kk * 2048, TC_HALF_BYTES, 1024);
-          umma_bf16(tmem_O, da, db, IDESC_PV, (j > 0 || kk > 0) ? 1u : 0u);
-        }
-        if (rowsum_mma) {
-          // row sums on the tensor core: L += P x ones[128 kv x 16] (every element 1.0, so only the footprint of the
-          // B operand matters: 4 core matrices = 512 B), which takes the 32 adds per thread and tile off the FMA pipe
-          // and makes the normaliser the sum of the ROUNDED probabilities
-          constexpr uint32_t IDESC_L = umma_idesc_n(16u, false, sizeof(ET) == 2 && !std::is_same<ET, __nv_bfloat16>::value);
-          const uint64_t dones = umma_desc_noswizzle(sQ_a + TC_ONES_OFFSET, 128, 256);
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {
-            const uint64_t da = umma_desc(sK_a(s) + (kk >> 2) * TC_HALF_BYTES + (kk & 3) * 32, 16, 1024);
-            umma_bf16(tmem_L, da, dones, IDESC_L, (j > 0 || kk > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(BAR(B_FREE + s));
-        if (j == my_tiles - 1) umma_commit(BAR(B_OFINAL));
-      }
-    }
-    __syncwarp();
-  } else {
-    // ================= softmax: four threads per query row =================
-    // Warp w (2..17): TMEM quadrant (w & 3) = 32 rows, column quarter (w - 2) >> 2 = 32 of the tile's 128 kv
-    // columns.  The four threads of a row meet once per tile (row max, exchanged as bf16 -- the rounded max
-    // is exactly what the reference's rounding points produce) through smem + a named barrier.
-    const int quad = warp & 3;
-    const int q4 = (warp - 2) >> 2;
-    const int row_l = quad * 32 + lane;             // TMEM lane == row inside the tile
-    const int row = mt * TC_BM + row_l;             // step-local row
-    const uint32_t* mrow = (row < q_pad && !is_prefill && rowmask != nullptr) ? rowmask + (long long)row * mask_words : nullptr;
-    const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
-    const uint32_t tO = tmem_O + lane_addr + (uint32_t)q4 * 32u;
-    float m_used = -INFINITY, l_sum = 0.f;
-    for (int j = 0; j < my_tiles; ++j) {
-      const int buf = j & 1, s = j % nst;
-      if (j == 1) TC_STAMP(8, 64);
-      mbar_wait(BAR(B_SFULL + buf), (j >> 1) & 1);
-      tc_fence_after();
-      if (j == 0) TC_STAMP(TS_SFULL0, 64);
-      if (j == 1) TC_STAMP(9, 64);
-      const int col0 = (tile_lo + j) * TC_BN + q4 * 32;
-      uint32_t mb = 0xffffffffu;
-      if (col0 + 32 > kv_len) mb = visible_bits32(mrow, mask_words, col0, kv_len, q_len, is_prefill, row);
-      float v[32];
-      tmem_ld32(tmem_base + lane_addr + (uint32_t)buf * 128u + (uint32_t)q4 * 32u, v);
-      tmem_ld_wait();
-      if (j == 1) TC_STAMP(10, 64);
-      // row max of my 32 columns; bf16 rounding and the positive scale are monotone, so round the max once
-      float mq[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};   // four independent chains
-      if (__all_sync(0xffffffffu, mb == 0xffffffffu)) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mq[i & 3] = fmaxf(mq[i & 3], v[i]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mq[i & 3] = fmaxf(mq[i & 3], ((mb >> i) & 1u) ? v[i] : -INFINITY);
-      }
-      const float mx_raw = fmaxf(fmaxf(mq[0], mq[1]), fmaxf(mq[2], mq[3]));
-      ET* xm = s_xmax + (j & 1) * 512;   // slot parity: no write-after-read race across tiles
-      xm[q4 * 128 + row_l] = Elem<ET>::from_f(mx_raw == -INFINITY ? -INFINITY : round_to<ET>(mx_raw) * inv_sqrt_d);
-      if (j == 1) TC_STAMP(11, 64);
-      named_bar_sync(1, TC_SOFTMAX_THREADS);
-      if (j == 1) TC_STAMP(12, 64);
-      const float mx = fmaxf(fmaxf(Elem<ET>::to_f(xm[row_l]), Elem<ET>::to_f(xm[128 + row_l])),
-                             fmaxf(Elem<ET>::to_f(xm[256 + row_l]), Elem<ET>::to_f(xm[384 + row_l])));
-      // lazy rescale: keep the stale max while it is within 2^8 of the running max (all four threads agree)
-      if (j == 0) {
-        m_used = mx;
-      } else {
-        const bool need = (mx > m_used + 5.545177f) || (m_used == -INFINITY && mx > -INFINITY);
-        if (__any_sync(0xffffffffu, need)) {
-          mbar_wait(BAR(B_FREE + (j - 1) % nst), ((j - 1) / nst) & 1);   // PV(j-1) landed in O
-          tc_fence_after();
-          const float m_new = fmaxf(m_used, mx);
-          const float scale = (m_new == -INFINITY) ? 1.f : exp2f((m_used - m_new) * TC_LOG2E);
-          l_sum *= scale;
-          tmem_ld32(tO, ov);                         // my quarter of the O columns
-          float lv = 0.f;
-          if (rowsum_mma && q4 == 0) lv = tmem_ld1(tmem_L + lane_addr);      // ... and the row's running sum
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) ov[i] *= scale;
-          tmem_st32(tO, ov);
-          if (rowsum_mma && q4 == 0) tmem_st1(tmem_L + lane_addr, lv * scale);
-          tmem_st_wait();
-          m_used = m_new;
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+
+  if (warp == 8) {
+    // ================= TMA producer (tiles beyond the first STAGES; the rest was issued above) =================
+    if (active) {
+      if (lane == 0) {
+        for (int j = TC_STAGES; j < my_tiles; ++j) {
+          const int s = j % TC_STAGES;
+          mbar_wait(BAR(B_FREE + s), ((j / TC_STAGES) - 1) & 1);
+          issue_tile(j);
         }
       }
-      const float off = (m_used == -INFINITY) ? 0.f : m_used * TC_LOG2E;
-      // P = exp2(score - max) as bf16 into the K stage, K-major SWIZZLE_128B:
-      //   [kv block of 64][row][128 B], 16-byte chunk index ^ (row & 7); my quarter = 4 chunks of block q4 / 2
-      unsigned char* prow = smem + TC_TILE_BYTES * (1 + 2 * s) + (q4 >> 1) * TC_HALF_BYTES + row_l * 128;
-      // warp-uniform choice: chunks made of cache columns only (all but the last 1-2 tiles) run a loop with no
-      // mask instructions at all -- the softmax warps are issue-bound, every instruction per element counts
-      const bool all_vis = __all_sync(0xffffffffu, mb == 0xffffffffu);
-      float ps4[4] = {0.f, 0.f, 0.f, 0.f};
-      if (all_vis) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float p[8];
-#pragma unroll
-          for (int e = 0; e < 8; e += 2) {
-            const int i = g * 8 + e;
-            // reference rounding points, two elements per cvt: bf16(bf16(s) * (1/sqrt(d))).  The halves are unpacked
-            // by hand (one shift, one mask): __bfloat1622float2 costs an extra PRMT per pair.
-            float r0, r1;
-            round_scale_round2<ET>(v[i], v[i + 1], inv_sqrt_d, r0, r1);
-            p[e] = ex2_approx(r0 * TC_LOG2E - off);
-            p[e + 1] = ex2_approx(r1 * TC_LOG2E - off);
-            if (!rowsum_mma) ps4[g] += p[e] + p[e + 1];
-          }
-          uint4 pk;
-          pk.x = Elem<ET>::pack2(p[0], p[1]); pk.y = Elem<ET>::pack2(p[2], p[3]);
-          pk.z = Elem<ET>::pack2(p[4], p[5]); pk.w = Elem<ET>::pack2(p[6], p[7]);
-          const int cc = (q4 & 1) * 4 + g;
-          *reinterpret_cast<uint4*>(prow + ((cc ^ (row_l & 7)) << 4)) = pk;
-        }
-      } else {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float p[8];
-#pragma unroll
-          for (int e = 0; e < 8; e += 2) {
-            const int i = g * 8 + e;
-            float r0, r1;
-            round_scale_round2<ET>(v[i], v[i + 1], inv_sqrt_d, r0, r1);
-            p[e] = ((mb >> i) & 1u) ? ex2_approx(r0 * TC_LOG2E - off) : 0.f;
-            p[e + 1] = ((mb >> (i + 1)) & 1u) ? ex2_approx(r1 * TC_LOG2E - off) : 0.f;
-            if (!rowsum_mma) ps4[g] += p[e] + p[e + 1];
-          }
-          uint4 pk;
-          pk.x = Elem<ET>::pack2(p[0], p[1]); pk.y = Elem<ET>::pack2(p[2], p[3]);
-          pk.z = Elem<ET>::pack2(p[4], p[5]); pk.w = Elem<ET>::pack2(p[6], p[7]);
-          const int cc = (q4 & 1) * 4 + g;
-          *reinterpret_cast<uint4*>(prow + ((cc ^ (row_l & 7)) << 4)) = pk;
-        }
-      }
-      if (!rowsum_mma) l_sum += (ps4[0] + ps4[1]) + (ps4[2] + ps4[3]);
-      if (j == 1) TC_STAMP(13, 64);
-      // stale cache rows past T must not reach the PV MMA (0 * NaN): zero them in the staged V tile
-      const int tile0 = (tile_lo + j) * TC_BN;
-      if (tile0 + TC_BN > T) {
-        mbar_wait(BAR(B_VFULL + s), (j / nst) & 1);
-        if (tile0 + row_l >= T) {                   // V tile row == kv row; each quarter clears 64 of its 256 bytes
-          unsigned char* pV = smem + TC_TILE_BYTES * (2 + 2 * s) + (q4 >> 1) * TC_HALF_BYTES + row_l * 128 + (q4 & 1) * 64;
-          const uint4 z = make_uint4(0, 0, 0, 0);
-#pragma unroll
-          for (int cc = 0; cc < 4; ++cc) *reinterpret_cast<uint4*>(pV + cc * 16) = z;
-        }
-      }
-      fence_proxy_async();                         // my P / V writes -> visible to the tensor core's async proxy
-      tc_fence_before();
-      if (j == 1) TC_STAMP(14, 64);
       __syncwarp();
-      if (lane == 0) mbar_arrive(BAR(B_PFULL + buf));   // one arrival per warp (16), not 512 smem atomics
-      if (j == 1) TC_STAMP(15, 64);
-    }
-
-    // ---- epilogue: row sums meet; O (TMEM) -> registers.  Single split: normalise and store.  Split-KV: the registers
-    // are pushed to the owner CTA of the row after the role branches join (tail of the kernel).
-    mbar_wait(BAR(B_OFINAL), 0);
-    tc_fence_after();
-    TC_STAMP(TS_OFINAL, 64);
-    if (rowsum_mma) {
-      l_sum = tmem_ld1(tmem_L + lane_addr);         // every thread of the row reads the row's sum
-    } else {
-      named_bar_sync(1, TC_SOFTMAX_THREADS);        // the max-exchange slots are free again
-      s_xsum[q4 * 128 + row_l] = l_sum;
-      named_bar_sync(1, TC_SOFTMAX_THREADS);
-      l_sum = (s_xsum[row_l] + s_xsum[128 + row_l]) + (s_xsum[256 + row_l] + s_xsum[384 + row_l]);
-    }
-    tmem_ld32(tO, ov);
-    tmem_ld_wait();
-    m_row = m_used;
-    l_row = l_sum;
-    if (n_splits == 1) {
-      const float inv = l_sum > 0.f ? 1.f / l_sum : 0.f;
-      if (row < q_pad) {
-        uint4* dst = reinterpret_cast<uint4*>(out + (long long)row * HD + h * TC_D + q4 * 32);
-#pragma unroll
-        for (int v4 = 0; v4 < 4; ++v4) {
-          uint4 pk;
-          pk.x = Elem<ET>::pack2(ov[v4 * 8 + 0] * inv, ov[v4 * 8 + 1] * inv);
-          pk.y = Elem<ET>::pack2(ov[v4 * 8 + 2] * inv, ov[v4 * 8 + 3] * inv);
-          pk.z = Elem<ET>::pack2(ov[v4 * 8 + 4] * inv, ov[v4 * 8 + 5] * inv);
-          pk.w = Elem<ET>::pack2(ov[v4 * 8 + 6] * inv, ov[v4 * 8 + 7] * inv);
-          dst[v4] = pk;
+      if (zero_last) {
+        const int j = my_tiles - 1, s = j % TC_STAGES;
+        const int r0 = T - (tile_lo + j) * TC_BN;      // first stale row of the tile
+        mbar_wait(BAR(B_VFULL + s), (j / TC_STAGES) & 1);
+        unsigned char* pV = smem + TC_TILE_BYTES * (2 + 2 * s);
+        const uint4 z = make_uint4(0, 0, 0, 0);
+        for (int c = r0 * 8 + lane; c < TC_BN * 8; c += 32) {      // whole 128-byte rows: the swizzle does not matter
+          const int r = c >> 3, cc = c & 7;
+          *reinterpret_cast<uint4*>(pV + r * 128 + cc * 16) = z;
+          *reinterpret_cast<uint4*>(pV + TC_HALF_BYTES + r * 128 + cc * 16) = z;
         }
+        fence_proxy_async();                          // the zeros -> visible to the tensor core's async proxy
+        __syncwarp();
+        if (lane == 0) mbar_arrive(BAR(B_VZERO));
       }
     }
-    tc_fence_before();
-  }
-
-  // ---- teardown (TMEM) ----
-  if (active) {
-    __syncthreads();
-    if (warp == 1) {
-      tc_fence_after();
-      tmem_dealloc(tmem_base, 512);
+    if (REF) {                                        // meet the cluster at the row-max and row-sum exchanges
+      cluster_arrive(); cluster_wait();
+      cluster_arrive(); cluster_wait();
+    }
+  } else {
+    const int row[2] = {mt * TC_BM + rl[0], mt * TC_BM + rl[1]};   // step-local rows
+    const uint32_t* const mrow[2] = {
+        (row[0] < q_pad && !is_prefill && rowmask != nullptr) ? rowmask + (long long)row[0] * mask_words : nullptr,
+        (row[1] < q_pad && !is_prefill && rowmask != nullptr) ? rowmask + (long long)row[1] * mask_words : nullptr};
+    auto wait_v = [&](int j) {
+      const int s = j % TC_STAGES;
+      mbar_wait(BAR(B_VFULL + s), (j / TC_STAGES) & 1);
+      if (zero_last && j == my_tiles - 1) mbar_wait(BAR(B_VZERO), 0);
+    };
+    if (work) mbar_wait(BAR(B_QFULL), 0);
+    if (!REF) {
+      // ================= online softmax: one pass over the split's tiles =================
+      for (int j = 0; work && j < my_tiles; ++j) {
+        const int s = j % TC_STAGES;
+        const int tile0 = (tile_lo + j) * TC_BN;
+        mbar_wait(BAR(B_KFULL + s), (j / TC_STAGES) & 1);
+        if (j == 0) TC_STAMP(TS_KFULL0, 0);
+        float sc[64];
+        qk_tile<ET>(sc, sQ_a, sK_a(s), wg);
+        if (j == 0) TC_STAMP(TS_SFULL0, 0);
+        uint32_t mb[2][4];
+        tile_mask(mb, mrow, row, mask_words, tile0, kv_len, q_len, is_prefill);
+        // row max of the raw scores; bf16 rounding and the positive scale are monotone, so round the max once
+        float off[2];
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          float mx = -INFINITY;
+#pragma unroll
+          for (int i = 0; i < 16; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) mx = fmaxf(mx, vis(mb, rr, i, e, t) ? sc[4 * i + 2 * rr + e] : -INFINITY);
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          const float mtile = mx == -INFINITY ? -INFINITY : round_to<ET>(round_to<ET>(mx) * inv_sqrt_d);
+          if (mtile > m_row[rr]) {                    // the running max grew: rescale what was accumulated so far
+            const float scale = m_row[rr] == -INFINITY ? 1.f : exp2f((m_row[rr] - mtile) * TC_LOG2E);
+            l_row[rr] *= scale;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) { o[4 * i + 2 * rr] *= scale; o[4 * i + 2 * rr + 1] *= scale; }
+            m_row[rr] = mtile;
+          }
+          off[rr] = m_row[rr] == -INFINITY ? 0.f : m_row[rr] * TC_LOG2E;
+        }
+        // P = exp2(score - max) in the model dtype, straight into the A fragments of P.V; the row sum adds the ROUNDED
+        // probabilities (the normaliser of exactly what the MMA multiplies)
+        uint32_t pa[32];
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            float r0, r1;
+            round_scale_round2<ET>(sc[4 * i + 2 * rr], sc[4 * i + 2 * rr + 1], inv_sqrt_d, r0, r1);
+            const float p0 = vis(mb, rr, i, 0, t) ? ex2_approx(r0 * TC_LOG2E - off[rr]) : 0.f;
+            const float p1 = vis(mb, rr, i, 1, t) ? ex2_approx(r1 * TC_LOG2E - off[rr]) : 0.f;
+            const uint32_t pk = Elem<ET>::pack2(p0, p1);
+            const float2 pr = unpack2<ET>(pk);
+            l_row[rr] += pr.x + pr.y;
+            pa[4 * (i >> 1) + 2 * (i & 1) + rr] = pk;
+          }
+        wait_v(j);
+        pv_tile<ET>(o, pa, sV_a(s));
+        __syncwarp();
+        if (lane == 0) mbar_arrive(BAR(B_FREE + s));
+      }
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        l_row[rr] += __shfl_xor_sync(0xffffffffu, l_row[rr], 1);
+        l_row[rr] += __shfl_xor_sync(0xffffffffu, l_row[rr], 2);
+      }
+    } else {
+      // ================= reference order: row max, row sum, then P.V, S recomputed in each pass =================
+      float sc[64];
+      uint32_t mb[2][4];
+      // ---- pass A: the row maximum of the split
+      float mx[2] = {-INFINITY, -INFINITY};
+      for (int j = 0; work && j < my_tiles; ++j) {
+        mbar_wait(BAR(B_KFULL + j), 0);
+        qk_tile<ET>(sc, sQ_a, sK_a(j), wg);
+        tile_mask(mb, mrow, row, mask_words, (tile_lo + j) * TC_BN, kv_len, q_len, is_prefill);
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+          for (int i = 0; i < 16; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) mx[rr] = fmaxf(mx[rr], vis(mb, rr, i, e, t) ? sc[4 * i + 2 * rr + e] : -INFINITY);
+      }
+      if (work) {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 1));
+          mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 2));
+          const float m_split = mx[rr] == -INFINITY ? -INFINITY : round_to<ET>(round_to<ET>(mx[rr]) * inv_sqrt_d);
+          if (t == 0) row_ml[(hm * n_splits + split) * TC_BM + rl[rr]].x = m_split;
+        }
+      }
+      cluster_arrive(); cluster_wait();
+      float m_ref[2] = {0.f, 0.f};
+      if (work) {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          float m_all = -INFINITY;
+          for (int sp = 0; sp < n_active; ++sp)
+            m_all = fmaxf(m_all, ld_global_f2(row_ml + (hm * n_splits + sp) * TC_BM + rl[rr]).x);
+          m_ref[rr] = (m_all == -INFINITY) ? 0.f : m_all;   // x - max is exact in fp32 (both are model-dtype values)
+        }
+      }
+      // e = exp(x - max) in fp32 of tile j (S recomputed from the resident K tile)
+      auto exps = [&](int j) {
+        qk_tile<ET>(sc, sQ_a, sK_a(j), wg);
+        tile_mask(mb, mrow, row, mask_words, (tile_lo + j) * TC_BN, kv_len, q_len, is_prefill);
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            float r0, r1;
+            round_scale_round2<ET>(sc[4 * i + 2 * rr], sc[4 * i + 2 * rr + 1], inv_sqrt_d, r0, r1);
+            sc[4 * i + 2 * rr] = vis(mb, rr, i, 0, t) ? ex2_approx((r0 - m_ref[rr]) * TC_LOG2E) : 0.f;
+            sc[4 * i + 2 * rr + 1] = vis(mb, rr, i, 1, t) ? ex2_approx((r1 - m_ref[rr]) * TC_LOG2E) : 0.f;
+          }
+      };
+      // ---- pass B: the row sum of the split
+      float l_part[2] = {0.f, 0.f};
+      for (int j = 0; work && j < my_tiles; ++j) {
+        exps(j);
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            l_part[rr] += sc[4 * i + 2 * rr];
+            l_part[rr] += sc[4 * i + 2 * rr + 1];
+          }
+      }
+      if (work) {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          l_part[rr] += __shfl_xor_sync(0xffffffffu, l_part[rr], 1);
+          l_part[rr] += __shfl_xor_sync(0xffffffffu, l_part[rr], 2);
+          if (t == 0) row_ml[(hm * n_splits + split) * TC_BM + rl[rr]].y = l_part[rr];
+        }
+      }
+      cluster_arrive(); cluster_wait();
+      float l_all[2] = {0.f, 0.f};
+      if (work) {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr)
+          for (int sp = 0; sp < n_active; ++sp) l_all[rr] += ld_global_f2(row_ml + (hm * n_splits + sp) * TC_BM + rl[rr]).y;
+      }
+      // ---- pass C: p = model_dtype(e / sum) -> P.V, tile by tile
+      for (int j = 0; work && j < my_tiles; ++j) {
+        exps(j);
+        uint32_t pa[32];
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const float p0 = l_all[rr] > 0.f ? __fdiv_rn(sc[4 * i + 2 * rr], l_all[rr]) : 0.f;
+            const float p1 = l_all[rr] > 0.f ? __fdiv_rn(sc[4 * i + 2 * rr + 1], l_all[rr]) : 0.f;
+            pa[4 * (i >> 1) + 2 * (i & 1) + rr] = Elem<ET>::pack2(p0, p1);
+          }
+        wait_v(j);
+        pv_tile<ET>(o, pa, sV_a(j));
+      }
+    }
+    TC_STAMP(TS_OFINAL, 0);
+    if (work && n_splits == 1) {
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        if (row[rr] >= q_pad) continue;
+        const float inv = REF ? 1.f : (l_row[rr] > 0.f ? 1.f / l_row[rr] : 0.f);
+        uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)row[rr] * HD + h * TC_D + 2 * t);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) dst[4 * i] = Elem<ET>::pack2(o[4 * i + 2 * rr] * inv, o[4 * i + 2 * rr + 1] * inv);
+      }
     }
   }
   TC_STAMP(TS_STAGED, 0);
   if (n_splits == 1) { TC_STAMP(TS_END, 0); return; }
 
   // ---- split merge across the cluster ----
-  // Row r of the tile is owned by CTA r / per (per = ceil(128 / n_active)).  Every softmax thread holds 32 fp32 of
-  // its split's unnormalised O row (and the row's (m, l)) in registers; threads of owned rows keep theirs, the others
-  // ship theirs to the owner, who combines:  w_s = 2^(m_s - m),  out = sum_s w_s O_s / sum_s w_s l_s.
-  // Transport 0 (LADE_ATTN_MERGE=l2, kept for A/B): the split's slab of an L2-resident scratch + one cluster barrier.
-  // only the tile's real rows (row < q_pad) travel: the padding rows of the last q tile are neither pushed nor merged
+  // Row r of the tile is owned by CTA r / per (per = ceil(rows / n_active)); only the tile's real rows (row < q_pad)
+  // travel.  Threads of foreign rows store their registers straight into the owner CTA's shared memory
+  // (st.shared::cluster, fire and forget); barrier 1 = every CTA is done with its stages, barrier 2 = the pushes have
+  // landed; the owner threads then combine their own registers with the slots from LOCAL shared memory:
+  //   impl 2:  w_s = 2^(m_s - m),  out = sum_s w_s O_s / sum_s w_s l_s        impl 3:  out = sum_s O_s
   const int rows_valid = min(TC_BM, q_pad - mt * TC_BM);
   const int per = (rows_valid + n_active - 1) / n_active;
-  int dest = -1;
-  const long long hm = (long long)h * gridDim.z + mt;
-  if (merge_mode == 1) {
-    // ---- default transport: PUSH through distributed shared memory ------------------------------------------------
-    // Threads of foreign rows store their 32 registers straight into the owner CTA's shared memory (st.shared::cluster,
-    // fire and forget: no local staging, no dependent remote loads).  Slot k of an owner = [per][TC_SO_STRIDE] floats in
-    // its (dead) K/V stages; barrier 1 = every CTA is done with its stages, barrier 2 = the pushes have landed; the
-    // owner threads then combine their own registers with the slots from LOCAL shared memory.  Same-box A/B
-    // (profiles/r02_attn_merge_ab.jsonl): 15.2 us per launch at the bench shape against 18.6 us for the L2 transport
-    // below and 16.9 us for round 1's pull (stage locally, siblings read over DSMEM).
-    if (nst != 2) cluster_arrive();
-    cluster_wait();
-    TC_STAMP(TS_CLUSTER, 0);
-    int r_in = 0;
-    if (active && warp >= 2) {
-      const int row_l = (warp & 3) * 32 + lane;
-      const int q4 = (warp - 2) >> 2;
-      dest = row_l < rows_valid ? row_l / per : -2;
-      r_in = row_l - dest * per;
-      if (dest >= 0 && dest != split) {
-        const int slot = split < dest ? split : split - 1;
-        const uint32_t o_a = dsmem_addr(sQ_a + TC_SO_OFFSET + (uint32_t)(((slot * per + r_in) * TC_SO_STRIDE + q4 * 32) * 4), dest);
+  cluster_arrive();
+  cluster_wait();
+  TC_STAMP(TS_CLUSTER, 0);
+  int dest[2] = {-1, -1}, r_in[2] = {0, 0};
+  if (work) {
 #pragma unroll
-        for (int v4 = 0; v4 < 8; ++v4) st_dsmem_f4(o_a + v4 * 16, ov[v4 * 4], ov[v4 * 4 + 1], ov[v4 * 4 + 2], ov[v4 * 4 + 3]);
-        if (q4 == 0) st_dsmem_f2(dsmem_addr(sQ_a + TC_SML_OFFSET + (uint32_t)((slot * per + r_in) * 8), dest), m_row, l_row);
+    for (int rr = 0; rr < 2; ++rr) {
+      dest[rr] = rl[rr] < rows_valid ? rl[rr] / per : -2;
+      r_in[rr] = rl[rr] - dest[rr] * per;
+      if (dest[rr] >= 0 && dest[rr] != split) {
+        const int slot = split < dest[rr] ? split : split - 1;
+        const uint32_t o_a = dsmem_addr(sQ_a + TC_SO_OFFSET + (uint32_t)(((slot * per + r_in[rr]) * TC_SO_STRIDE + 2 * t) * 4), dest[rr]);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) st_dsmem_f2(o_a + i * 32, o[4 * i + 2 * rr], o[4 * i + 2 * rr + 1]);
+        if (!REF && t == 0)
+          st_dsmem_f2(dsmem_addr(sQ_a + TC_SML_OFFSET + (uint32_t)((slot * per + r_in[rr]) * 8), dest[rr]), m_row[rr], l_row[rr]);
       }
-    }
-    cluster_arrive();
-    cluster_wait();
-    TC_STAMP(TS_MERGED, 0);
-    if (active && warp >= 2 && dest == split) {
-      const int row_l = (warp & 3) * 32 + lane;
-      const int q4 = (warp - 2) >> 2;
-      const int row = mt * TC_BM + row_l;
-      const float2* sml = reinterpret_cast<const float2*>(smem + TC_SML_OFFSET);
-      const float* so = reinterpret_cast<const float*>(smem + TC_SO_OFFSET);
-      float mmax = m_row;
-      for (int k = 0; k < n_active - 1; ++k) mmax = fmaxf(mmax, sml[k * per + r_in].x);
-      float wgt = (m_row == -INFINITY) ? 0.f : exp2f((m_row - mmax) * TC_LOG2E);
-      float lsum = l_row * wgt;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) ov[i] *= wgt;
-      for (int k = 0; k < n_active - 1; ++k) {
-        const float2 ml = sml[k * per + r_in];
-        wgt = (ml.x == -INFINITY) ? 0.f : exp2f((ml.x - mmax) * TC_LOG2E);
-        lsum += ml.y * wgt;
-        const float4* src = reinterpret_cast<const float4*>(so + (k * per + r_in) * TC_SO_STRIDE + q4 * 32);
-#pragma unroll
-        for (int v4 = 0; v4 < 8; ++v4) {
-          const float4 x = src[v4];
-          ov[v4 * 4] += x.x * wgt; ov[v4 * 4 + 1] += x.y * wgt; ov[v4 * 4 + 2] += x.z * wgt; ov[v4 * 4 + 3] += x.w * wgt;
-        }
-      }
-      const float inv = lsum > 0.f ? 1.f / lsum : 0.f;
-      if (row < q_pad) {
-        uint4* dst = reinterpret_cast<uint4*>(out + (long long)row * HD + h * TC_D + q4 * 32);
-#pragma unroll
-        for (int v4 = 0; v4 < 4; ++v4) {
-          uint4 pk;
-          pk.x = Elem<ET>::pack2(ov[v4 * 8 + 0] * inv, ov[v4 * 8 + 1] * inv);
-          pk.y = Elem<ET>::pack2(ov[v4 * 8 + 2] * inv, ov[v4 * 8 + 3] * inv);
-          pk.z = Elem<ET>::pack2(ov[v4 * 8 + 4] * inv, ov[v4 * 8 + 5] * inv);
-          pk.w = Elem<ET>::pack2(ov[v4 * 8 + 6] * inv, ov[v4 * 8 + 7] * inv);
-          dst[v4] = pk;
-        }
-      }
-    }
-    TC_STAMP(TS_END, 0);
-    return;
-  }
-  if (active && warp >= 2) {
-    const int row_l = (warp & 3) * 32 + lane;
-    const int q4 = (warp - 2) >> 2;
-    dest = row_l < rows_valid ? row_l / per : -2;
-    if (dest >= 0 && dest != split) {
-      float4* dst = reinterpret_cast<float4*>(part_o + ((hm * n_splits + split) * TC_BM + row_l) * TC_D + q4 * 32);
-#pragma unroll
-      for (int v4 = 0; v4 < 8; ++v4) dst[v4] = make_float4(ov[v4 * 4], ov[v4 * 4 + 1], ov[v4 * 4 + 2], ov[v4 * 4 + 3]);
-      if (q4 == 0) part_ml[(hm * n_splits + split) * TC_BM + row_l] = make_float2(m_row, l_row);
     }
   }
   cluster_arrive();
   cluster_wait();
   TC_STAMP(TS_MERGED, 0);
-  if (active && warp >= 2 && dest == split) {
-    const int row_l = (warp & 3) * 32 + lane;
-    const int q4 = (warp - 2) >> 2;
-    const int row = mt * TC_BM + row_l;
-    float2 ml[7];
-    float mmax = m_row;
+  if (work) {
+    const float2* sml = reinterpret_cast<const float2*>(smem + TC_SML_OFFSET);
+    const float* so = reinterpret_cast<const float*>(smem + TC_SO_OFFSET);
 #pragma unroll
-    for (int k = 0; k < 7; ++k) {
-      const int sp = k < split ? k : k + 1;                     // the siblings, skipping myself
-      ml[k] = make_float2(-INFINITY, 0.f);
-      if (sp < n_active) ml[k] = ld_global_f2(part_ml + (hm * n_splits + sp) * TC_BM + row_l);
-      mmax = fmaxf(mmax, ml[k].x);
-    }
-    float wgt = (m_row == -INFINITY) ? 0.f : exp2f((m_row - mmax) * TC_LOG2E);
-    float lsum = l_row * wgt;
+    for (int rr = 0; rr < 2; ++rr) {
+      if (dest[rr] != split) continue;
+      float inv = 1.f;
+      if (!REF) {
+        float mmax = m_row[rr];
+        for (int k = 0; k < n_active - 1; ++k) mmax = fmaxf(mmax, sml[k * per + r_in[rr]].x);
+        float wgt = (m_row[rr] == -INFINITY) ? 0.f : exp2f((m_row[rr] - mmax) * TC_LOG2E);
+        float lsum = l_row[rr] * wgt;
 #pragma unroll
-    for (int i = 0; i < 32; ++i) ov[i] *= wgt;
+        for (int i = 0; i < 16; ++i) { o[4 * i + 2 * rr] *= wgt; o[4 * i + 2 * rr + 1] *= wgt; }
+        for (int k = 0; k < n_active - 1; ++k) {
+          const float2 ml = sml[k * per + r_in[rr]];
+          wgt = (ml.x == -INFINITY) ? 0.f : exp2f((ml.x - mmax) * TC_LOG2E);
+          lsum += ml.y * wgt;
+          const float* src = so + (k * per + r_in[rr]) * TC_SO_STRIDE + 2 * t;
 #pragma unroll
-    for (int k = 0; k < 7; ++k) {
-      const int sp = k < split ? k : k + 1;
-      if (sp >= n_active) continue;
-      wgt = (ml[k].x == -INFINITY) ? 0.f : exp2f((ml[k].x - mmax) * TC_LOG2E);
-      lsum += ml[k].y * wgt;
-      const float* src = part_o + ((hm * n_splits + sp) * TC_BM + row_l) * TC_D + q4 * 32;
-      float4 x[8];
+          for (int i = 0; i < 16; ++i) {
+            const float2 x = *reinterpret_cast<const float2*>(src + 8 * i);
+            o[4 * i + 2 * rr] += x.x * wgt;
+            o[4 * i + 2 * rr + 1] += x.y * wgt;
+          }
+        }
+        inv = lsum > 0.f ? 1.f / lsum : 0.f;
+      } else {
+        for (int k = 0; k < n_active - 1; ++k) {
+          const float* src = so + (k * per + r_in[rr]) * TC_SO_STRIDE + 2 * t;
 #pragma unroll
-      for (int v4 = 0; v4 < 8; ++v4) x[v4] = ld_global_f4(src + v4 * 4);
-#pragma unroll
-      for (int v4 = 0; v4 < 8; ++v4) {
-        ov[v4 * 4] += x[v4].x * wgt; ov[v4 * 4 + 1] += x[v4].y * wgt; ov[v4 * 4 + 2] += x[v4].z * wgt; ov[v4 * 4 + 3] += x[v4].w * wgt;
+          for (int i = 0; i < 16; ++i) {
+            const float2 x = *reinterpret_cast<const float2*>(src + 8 * i);
+            o[4 * i + 2 * rr] += x.x;
+            o[4 * i + 2 * rr + 1] += x.y;
+          }
+        }
       }
-    }
-    const float inv = lsum > 0.f ? 1.f / lsum : 0.f;
-    if (row < q_pad) {
-      uint4* dst = reinterpret_cast<uint4*>(out + (long long)row * HD + h * TC_D + q4 * 32);
+      const int row = mt * TC_BM + rl[rr];
+      if (row < q_pad) {
+        uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)row * HD + h * TC_D + 2 * t);
 #pragma unroll
-      for (int v4 = 0; v4 < 4; ++v4) {
-        uint4 pk;
-        pk.x = Elem<ET>::pack2(ov[v4 * 8 + 0] * inv, ov[v4 * 8 + 1] * inv);
-        pk.y = Elem<ET>::pack2(ov[v4 * 8 + 2] * inv, ov[v4 * 8 + 3] * inv);
-        pk.z = Elem<ET>::pack2(ov[v4 * 8 + 4] * inv, ov[v4 * 8 + 5] * inv);
-        pk.w = Elem<ET>::pack2(ov[v4 * 8 + 6] * inv, ov[v4 * 8 + 7] * inv);
-        dst[v4] = pk;
+        for (int i = 0; i < 16; ++i) dst[4 * i] = Elem<ET>::pack2(o[4 * i + 2 * rr] * inv, o[4 * i + 2 * rr + 1] * inv);
       }
     }
   }
   TC_STAMP(TS_END, 0);
-}
-
-// ---- reference-order variant (impl 3) ---------------------------------------------------------------------
-// Same tiles, same MMAs, same split over a cluster -- but the probabilities are rounded the way the reference rounds
-// them (lade/models/modeling_llama.py:530-541): p = model_dtype( exp(x - max_row) / sum_row ) with the max and the sum
-// of the WHOLE row (all KV splits), normalised in fp32 BEFORE the rounding, then P.V with fp32 accumulation.  The
-// online-softmax kernel above has to round exp(x - max_so_far) before it knows the sum, which changes the last bit of
-// about half of the outputs (DESIGN.md 6).  Knowing the whole row first means: every S tile of a split stays resident
-// in tensor memory (3 x 128 columns + O = the 512 columns of an SM, so at most 3 KV tiles per split), and the splits
-// of a head meet twice in the middle of the kernel (row maxima, then row sums, through an L2-resident table and a
-// cluster barrier each).  It is an opt-in parity mode (impl = 3, `LookaheadEngine(attn_impl=3)`): slower, and bounded
-// to kv_len + q_len <= 384 * n_splits.
-template <typename ET>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-attn_fwd_tc_exact_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                         const __grid_constant__ CUtensorMap tmV, ET* __restrict__ out,
-                         const uint32_t* __restrict__ rowmask, int mask_words, const int* __restrict__ meta, int q_pad,
-                         int n_heads, int n_kv_heads, int n_splits, float inv_sqrt_d, float2* __restrict__ row_ml) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  const int split = blockIdx.x, h = blockIdx.y, mt = blockIdx.z;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q_len = meta[LADE_M_Q_LEN];
-  const int kv_len = meta[LADE_M_KV_LEN];
-  const int is_prefill = meta[LADE_M_IS_PREFILL];
-  const int T = kv_len + q_len;
-  int Tm = T;
-  if (is_prefill) Tm = min(T, kv_len + min(q_len, (mt + 1) * TC_BM));
-  const int n_tiles = (Tm + TC_BN - 1) / TC_BN;
-  const int t_base = n_tiles / n_splits, t_rem = n_tiles - t_base * n_splits;
-  const int n_active = n_tiles < n_splits ? n_tiles : n_splits;
-  const bool active = split < n_active;
-  const int tile_lo = split * t_base + (split < t_rem ? split : t_rem);
-  const int my_tiles = active ? t_base + (split < t_rem ? 1 : 0) : 0;
-  if (t_base + (t_rem ? 1 : 0) > 3) __trap();     // the caller's kv_bound was not a bound (host checks it)
-  const int hk = h / (n_heads / n_kv_heads);
-  const int HD = n_heads * TC_D;
-  const long long hm = (long long)h * gridDim.z + mt;
-  griddep_launch_dependents();
-
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_SMEM_TILES);
-  const uint32_t bar0 = smem_u32(bars);
-  auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  // barrier slots: 0 q_full | 1..3 k_full | 4..6 v_full | 7..9 s_full | 10..12 p_full | 13 o_final
-  const int B_QFULL = 0, B_KFULL = 1, B_VFULL = 4, B_SFULL = 7, B_PFULL = 10, B_OFINAL = 13;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 24);
-  ET* s_xmax = reinterpret_cast<ET*>(smem + TC_SMEM_TILES + 256);        // [4][128] row maxima of the four column quarters
-  float* s_xsum = reinterpret_cast<float*>(smem + TC_SMEM_TILES + 256);   // [4][128] row sums (after the maxima are dead)
-  const uint32_t sQ_a = smem_u32(smem);
-  auto sK_a = [&](int s) { return sQ_a + (uint32_t)TC_TILE_BYTES * (1 + 2 * s); };
-  auto sV_a = [&](int s) { return sQ_a + (uint32_t)TC_TILE_BYTES * (2 + 2 * s); };
-
-  if (active) {
-    if (threadIdx.x == 0) {
-      if ((sQ_a & 1023u) != 0) __trap();
-      mbar_init(BAR(B_QFULL), 1);
-      for (int s = 0; s < 3; ++s) {
-        mbar_init(BAR(B_KFULL + s), 1); mbar_init(BAR(B_VFULL + s), 1);
-        mbar_init(BAR(B_SFULL + s), 1); mbar_init(BAR(B_PFULL + s), TC_SOFTMAX_THREADS / 32);
-      }
-      mbar_init(BAR(B_OFINAL), 1);
-      fence_barrier_init();
-      auto issue_tile = [&](int j) {
-        const int row0 = (tile_lo + j) * TC_BN;
-        mbar_expect_tx(BAR(B_KFULL + j), TC_TILE_BYTES);
-        tma_load_3d(sK_a(j), &tmK, BAR(B_KFULL + j), 0, row0, hk);
-        tma_load_3d(sK_a(j) + TC_HALF_BYTES, &tmK, BAR(B_KFULL + j), 64, row0, hk);
-        mbar_expect_tx(BAR(B_VFULL + j), TC_TILE_BYTES);
-        tma_load_3d(sV_a(j), &tmV, BAR(B_VFULL + j), 0, row0, hk);
-        tma_load_3d(sV_a(j) + TC_HALF_BYTES, &tmV, BAR(B_VFULL + j), 64, row0, hk);
-      };
-      int n_old = 0;                                   // leading tiles that hold only rows of earlier steps
-      while (n_old < my_tiles && (tile_lo + n_old + 1) * TC_BN <= kv_len) ++n_old;
-      for (int j = 0; j < n_old; ++j) issue_tile(j);
-      griddep_wait();
-      mbar_expect_tx(BAR(B_QFULL), TC_TILE_BYTES);
-      tma_load_3d(sQ_a, &tmQ, BAR(B_QFULL), 0, mt * TC_BM, h);
-      tma_load_3d(sQ_a + TC_HALF_BYTES, &tmQ, BAR(B_QFULL), 64, mt * TC_BM, h);
-      for (int j = n_old; j < my_tiles; ++j) issue_tile(j);
-    }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-  }
-  const uint32_t tmem_base = active ? *tmem_slot : 0u;
-  const uint32_t tmem_O = tmem_base + 384;
-  float ov[32];                         // a softmax thread's share of its split's (already normalised) partial O row
-
-  if (!active || warp == 0) {
-    // nothing to compute (idle split / the producer, whose loads are all in flight): meet the cluster twice
-    cluster_arrive(); cluster_wait();
-    cluster_arrive(); cluster_wait();
-  } else if (warp == 1) {
-    constexpr uint32_t IDESC_QK = umma_idesc<ET>(false);
-    constexpr uint32_t IDESC_PV = umma_idesc<ET>(true);
-    if (lane == 0) {
-      mbar_wait(BAR(B_QFULL), 0);
-      for (int j = 0; j < my_tiles; ++j) {
-        mbar_wait(BAR(B_KFULL + j), 0);
-        tc_fence_after();
-        const uint32_t d = tmem_base + (uint32_t)j * 128u;
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t da = umma_desc(sQ_a + kb * TC_HALF_BYTES + k * 32, 16, 1024);
-            const uint64_t db = umma_desc(sK_a(j) + kb * TC_HALF_BYTES + k * 32, 16, 1024);
-            umma_bf16(d, da, db, IDESC_QK, (kb | k) ? 1u : 0u);
-          }
-        umma_commit(BAR(B_SFULL + j));
-      }
-    }
-    __syncwarp();
-    cluster_arrive(); cluster_wait();     // row maxima of all splits
-    cluster_arrive(); cluster_wait();     // row sums of all splits
-    if (lane == 0) {
-      for (int j = 0; j < my_tiles; ++j) {
-        mbar_wait(BAR(B_PFULL + j), 0);
-        mbar_wait(BAR(B_VFULL + j), 0);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint64_t da = umma_desc(sK_a(j) + (kk >> 2) * TC_HALF_BYTES + (kk & 3) * 32, 16, 1024);
-          const uint64_t db = umma_desc(sV_a(j) + kk * 2048, TC_HALF_BYTES, 1024);
-          umma_bf16(tmem_O, da, db, IDESC_PV, (j > 0 || kk > 0) ? 1u : 0u);
-        }
-      }
-      umma_commit(BAR(B_OFINAL));
-    }
-    __syncwarp();
-  } else {
-    const int quad = warp & 3;
-    const int q4 = (warp - 2) >> 2;
-    const int row_l = quad * 32 + lane;
-    const int row = mt * TC_BM + row_l;
-    const uint32_t* mrow = (row < q_pad && !is_prefill && rowmask != nullptr) ? rowmask + (long long)row * mask_words : nullptr;
-    const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
-    const uint32_t tS = tmem_base + lane_addr + (uint32_t)q4 * 32u;
-    float v[32];
-    uint32_t mbits[3] = {0u, 0u, 0u};
-    // ---- pass A: the row maximum of the split (the rounding and the positive scale are monotone: round the max once)
-    float mx_raw = -INFINITY;
-    for (int j = 0; j < my_tiles; ++j) {
-      mbar_wait(BAR(B_SFULL + j), 0);
-      tc_fence_after();
-      const int col0 = (tile_lo + j) * TC_BN + q4 * 32;
-      uint32_t mb = 0xffffffffu;
-      if (col0 + 32 > kv_len) mb = visible_bits32(mrow, mask_words, col0, kv_len, q_len, is_prefill, row);
-      if (j == 0) mbits[0] = mb; else if (j == 1) mbits[1] = mb; else mbits[2] = mb;
-      tmem_ld32(tS + (uint32_t)j * 128u, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) mx_raw = fmaxf(mx_raw, ((mb >> i) & 1u) ? v[i] : -INFINITY);
-    }
-    s_xmax[q4 * 128 + row_l] = Elem<ET>::from_f(mx_raw == -INFINITY ? -INFINITY : round_to<ET>(mx_raw) * inv_sqrt_d);
-    named_bar_sync(1, TC_SOFTMAX_THREADS);
-    const float m_split = fmaxf(fmaxf(Elem<ET>::to_f(s_xmax[row_l]), Elem<ET>::to_f(s_xmax[128 + row_l])),
-                                fmaxf(Elem<ET>::to_f(s_xmax[256 + row_l]), Elem<ET>::to_f(s_xmax[384 + row_l])));
-    if (q4 == 0) row_ml[(hm * n_splits + split) * TC_BM + row_l].x = m_split;
-    cluster_arrive(); cluster_wait();
-    float m_all = -INFINITY;
-    for (int s = 0; s < n_active; ++s) m_all = fmaxf(m_all, ld_global_f2(row_ml + (hm * n_splits + s) * TC_BM + row_l).x);
-    const float m_ref = (m_all == -INFINITY) ? 0.f : m_all;   // x - max is exact in fp32 (both are model-dtype values)
-    // ---- pass B: e = exp(x - max) in fp32, kept in tensor memory in place of the scores; the row sum of the split
-    float l_part = 0.f;
-    for (int j = 0; j < my_tiles; ++j) {
-      const uint32_t mb = j == 0 ? mbits[0] : (j == 1 ? mbits[1] : mbits[2]);
-      tmem_ld32(tS + (uint32_t)j * 128u, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        float r0, r1;
-        round_scale_round2<ET>(v[i], v[i + 1], inv_sqrt_d, r0, r1);
-        v[i] = ((mb >> i) & 1u) ? ex2_approx((r0 - m_ref) * TC_LOG2E) : 0.f;
-        v[i + 1] = ((mb >> (i + 1)) & 1u) ? ex2_approx((r1 - m_ref) * TC_LOG2E) : 0.f;
-        l_part += v[i];
-        l_part += v[i + 1];
-      }
-      tmem_st32(tS + (uint32_t)j * 128u, v);
-      tmem_st_wait();
-    }
-    s_xsum[q4 * 128 + row_l] = l_part;      // the maxima were read by everybody before the cluster barrier above
-    named_bar_sync(1, TC_SOFTMAX_THREADS);
-    const float l_split = (s_xsum[row_l] + s_xsum[128 + row_l]) + (s_xsum[256 + row_l] + s_xsum[384 + row_l]);
-    if (q4 == 0) row_ml[(hm * n_splits + split) * TC_BM + row_l].y = l_split;
-    cluster_arrive(); cluster_wait();
-    float l_all = 0.f;
-    for (int s = 0; s < n_active; ++s) l_all += ld_global_f2(row_ml + (hm * n_splits + s) * TC_BM + row_l).y;
-    // ---- pass C: p = model_dtype(e / sum) -> the K stage (A operand of P.V), tile by tile
-    for (int j = 0; j < my_tiles; ++j) {
-      tmem_ld32(tS + (uint32_t)j * 128u, v);
-      tmem_ld_wait();
-      unsigned char* prow = smem + TC_TILE_BYTES * (1 + 2 * j) + (q4 >> 1) * TC_HALF_BYTES + row_l * 128;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        float p[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) p[e] = l_all > 0.f ? __fdiv_rn(v[g * 8 + e], l_all) : 0.f;
-        uint4 pk;
-        pk.x = Elem<ET>::pack2(p[0], p[1]); pk.y = Elem<ET>::pack2(p[2], p[3]);
-        pk.z = Elem<ET>::pack2(p[4], p[5]); pk.w = Elem<ET>::pack2(p[6], p[7]);
-        const int cc = (q4 & 1) * 4 + g;
-        *reinterpret_cast<uint4*>(prow + ((cc ^ (row_l & 7)) << 4)) = pk;
-      }
-      const int tile0 = (tile_lo + j) * TC_BN;
-      if (tile0 + TC_BN > T) {                       // stale cache rows past T must not reach the MMA (0 * NaN)
-        mbar_wait(BAR(B_VFULL + j), 0);
-        if (tile0 + row_l >= T) {
-          unsigned char* pV = smem + TC_TILE_BYTES * (2 + 2 * j) + (q4 >> 1) * TC_HALF_BYTES + row_l * 128 + (q4 & 1) * 64;
-          const uint4 z = make_uint4(0, 0, 0, 0);
-#pragma unroll
-          for (int cc = 0; cc < 4; ++cc) *reinterpret_cast<uint4*>(pV + cc * 16) = z;
-        }
-      }
-      fence_proxy_async();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(BAR(B_PFULL + j));
-    }
-    mbar_wait(BAR(B_OFINAL), 0);
-    tc_fence_after();
-    tmem_ld32(tmem_O + lane_addr + (uint32_t)q4 * 32u, ov);
-    tmem_ld_wait();
-    if (n_splits == 1 && row < q_pad) {
-      uint4* dst = reinterpret_cast<uint4*>(out + (long long)row * HD + h * TC_D + q4 * 32);
-#pragma unroll
-      for (int v4 = 0; v4 < 4; ++v4) {
-        uint4 pk;
-        pk.x = Elem<ET>::pack2(ov[v4 * 8 + 0], ov[v4 * 8 + 1]);
-        pk.y = Elem<ET>::pack2(ov[v4 * 8 + 2], ov[v4 * 8 + 3]);
-        pk.z = Elem<ET>::pack2(ov[v4 * 8 + 4], ov[v4 * 8 + 5]);
-        pk.w = Elem<ET>::pack2(ov[v4 * 8 + 6], ov[v4 * 8 + 7]);
-        dst[v4] = pk;
-      }
-    }
-    tc_fence_before();
-  }
-
-  if (active) {
-    __syncthreads();
-    if (warp == 1) {
-      tc_fence_after();
-      tmem_dealloc(tmem_base, 512);
-    }
-  }
-  if (n_splits == 1) return;
-
-  // ---- the partial rows of the splits are plain summands now: push to the owner, add, store (slots alias the stages)
-  const int rows_valid = min(TC_BM, q_pad - mt * TC_BM);
-  const int per = (rows_valid + n_active - 1) / n_active;
-  cluster_arrive(); cluster_wait();       // every CTA of the cluster is done with its K/V stages
-  int dest = -1, r_in = 0;
-  if (active && warp >= 2) {
-    const int row_l = (warp & 3) * 32 + lane;
-    const int q4 = (warp - 2) >> 2;
-    dest = row_l < rows_valid ? row_l / per : -2;
-    r_in = row_l - dest * per;
-    if (dest >= 0 && dest != split) {
-      const int slot = split < dest ? split : split - 1;
-      const uint32_t o_a = dsmem_addr(sQ_a + TC_TILE_BYTES + (uint32_t)(((slot * per + r_in) * TC_SO_STRIDE + q4 * 32) * 4), dest);
-#pragma unroll
-      for (int v4 = 0; v4 < 8; ++v4) st_dsmem_f4(o_a + v4 * 16, ov[v4 * 4], ov[v4 * 4 + 1], ov[v4 * 4 + 2], ov[v4 * 4 + 3]);
-    }
-  }
-  cluster_arrive(); cluster_wait();       // the pushes have landed
-  if (active && warp >= 2 && dest == split) {
-    const int row_l = (warp & 3) * 32 + lane;
-    const int q4 = (warp - 2) >> 2;
-    const int row = mt * TC_BM + row_l;
-    const float* so = reinterpret_cast<const float*>(smem + TC_TILE_BYTES);
-    for (int k = 0; k < n_active - 1; ++k) {
-      const float4* src = reinterpret_cast<const float4*>(so + (k * per + r_in) * TC_SO_STRIDE + q4 * 32);
-#pragma unroll
-      for (int v4 = 0; v4 < 8; ++v4) {
-        const float4 x = src[v4];
-        ov[v4 * 4] += x.x; ov[v4 * 4 + 1] += x.y; ov[v4 * 4 + 2] += x.z; ov[v4 * 4 + 3] += x.w;
-      }
-    }
-    if (row < q_pad) {
-      uint4* dst = reinterpret_cast<uint4*>(out + (long long)row * HD + h * TC_D + q4 * 32);
-#pragma unroll
-      for (int v4 = 0; v4 < 4; ++v4) {
-        uint4 pk;
-        pk.x = Elem<ET>::pack2(ov[v4 * 8 + 0], ov[v4 * 8 + 1]);
-        pk.y = Elem<ET>::pack2(ov[v4 * 8 + 2], ov[v4 * 8 + 3]);
-        pk.z = Elem<ET>::pack2(ov[v4 * 8 + 4], ov[v4 * 8 + 5]);
-        pk.w = Elem<ET>::pack2(ov[v4 * 8 + 6], ov[v4 * 8 + 7]);
-        dst[v4] = pk;
-      }
-    }
-  }
 }
 
 int attn_tc_set_timing_buffer(void* dev_ptr) {
@@ -910,35 +552,6 @@ static int get_tensor_map(const void* ptr, int rows, int heads, CUtensorMap* out
   return LADE_OK;
 }
 
-static int merge_mode() {          // default: DSMEM push (1); LADE_ATTN_MERGE=l2 selects the L2-scratch transport (0)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("LADE_ATTN_MERGE");
-    v = (e && e[0] == 'l') ? 0 : 1;
-  }
-  return v;
-}
-
-static int rowsum_mode() {         // default: row sums by an extra N=16 MMA against a ones tile; LADE_ATTN_ROWSUM=add: fp32 adds
-  static int v = -1;                 // same-box A/B (profiles/r02_attn_rowsum_ab.jsonl): 15.0 vs 15.2 us at the bench shape, 21.9 vs 22.5 at kv=3072
-  if (v < 0) {
-    const char* e = getenv("LADE_ATTN_ROWSUM");
-    v = (e && e[0] == 'a') ? 0 : 1;
-  }
-  return v;
-}
-
-static int stage2_tiles() {        // 2-deep K/V ring + dedicated merge slots when no split holds more tiles than this (0 = never)
-  static int v = -1;                 // same-box A/B (profiles/r02_attn_stage2_ab.jsonl): -2 ... -2.5 % up to 4 tiles per split, +2 % at 5
-  if (v < 0) {
-    const char* e = getenv("LADE_ATTN_STAGE2_TILES");
-    v = e ? atoi(e) : 4;
-    if (v < 0) v = 0;
-    if (v > 255) v = 255;
-  }
-  return v;
-}
-
 static int g_pdl_override = -1;      // lade_debug_attn_pdl: -1 = environment (LADE_PDL), 0 / 1 = forced
 int attn_tc_set_pdl(int v) { g_pdl_override = v < 0 ? -1 : (v ? 1 : 0); return LADE_OK; }
 
@@ -952,14 +565,12 @@ static bool pdl_enabled() {
   return v != 0;
 }
 
-template <typename ET>
-static int attn_fwd_tc_launch_t(cudaStream_t stream, const void* q, const void* k_cache, const void* v_cache, void* out,
-                                const uint32_t* rowmask, int mask_words, const int32_t* meta, void* scratch, int q_pad,
-                                int n_heads, int n_kv_heads, int head_dim, int kv_capacity, int kv_bound, int n_splits) {
-  (void)kv_bound;
-  if (head_dim != TC_D) return LADE_EUNSUPPORTED;
+// One launch of attn_fwd_tc_kernel<ET, REF>: grid (n_splits, heads, q tiles), the splits of a (head, q tile) a cluster.
+template <typename ET, bool REF>
+static int launch_tc(cudaStream_t stream, const void* q, const void* k_cache, const void* v_cache, void* out,
+                     const uint32_t* rowmask, int mask_words, const int32_t* meta, void* scratch, int q_pad, int n_heads,
+                     int n_kv_heads, int head_dim, int kv_capacity, int n_splits) {
   const int q_tiles = (q_pad + TC_BM - 1) / TC_BM;
-  if (n_splits > 8) n_splits = 8;   // portable cluster size
   if ((reinterpret_cast<uintptr_t>(q) & 15) || (reinterpret_cast<uintptr_t>(k_cache) & 15) ||
       (reinterpret_cast<uintptr_t>(v_cache) & 15))
     return LADE_EINVAL;
@@ -972,8 +583,7 @@ static int attn_fwd_tc_launch_t(cudaStream_t stream, const void* q, const void* 
   int cur_dev = 0;
   LADE_CUDA_CHECK(cudaGetDevice(&cur_dev));
   if (!((attr_devs >> (cur_dev & 63)) & 1ull)) {
-    LADE_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_tc_kernel<ET, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
-    LADE_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_tc_kernel<ET, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
+    LADE_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_tc_kernel<ET, REF>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
     attr_devs |= 1ull << (cur_dev & 63);
   }
   cudaLaunchConfig_t cfg = {};
@@ -993,16 +603,25 @@ static int attn_fwd_tc_launch_t(cudaStream_t stream, const void* q, const void* 
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 2 : 1;
   const float inv_sqrt_d = 1.0f / sqrtf((float)head_dim);
-  // scratch (lade_attn_scratch_bytes): [64 KB reserved][partial O: n_splits * n_heads * rows_pad * D fp32][(m, l) per row]
+  // scratch (lade_attn_scratch_bytes): [64 KB reserved][n_splits * n_heads * rows_pad * D fp32][(m, l) per row]; the
+  // reference-order variant exchanges its row maxima and sums through the (m, l) table
   float* part_o = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) + 65536);
-  float2* part_ml = reinterpret_cast<float2*>(part_o + (size_t)n_splits * n_heads * q_tiles * TC_BM * TC_D);
-  cudaError_t e = rowsum_mode()
-      ? cudaLaunchKernelEx(&cfg, attn_fwd_tc_kernel<ET, true>, tmQ, tmK, tmV, (ET*)out, rowmask, mask_words, meta,
-                           q_pad, n_heads, n_kv_heads, n_splits, inv_sqrt_d, part_o, part_ml, merge_mode() | (stage2_tiles() << 8))
-      : cudaLaunchKernelEx(&cfg, attn_fwd_tc_kernel<ET, false>, tmQ, tmK, tmV, (ET*)out, rowmask, mask_words, meta,
-                           q_pad, n_heads, n_kv_heads, n_splits, inv_sqrt_d, part_o, part_ml, merge_mode() | (stage2_tiles() << 8));
+  float2* row_ml = reinterpret_cast<float2*>(part_o + (size_t)n_splits * n_heads * q_tiles * TC_BM * TC_D);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, attn_fwd_tc_kernel<ET, REF>, tmQ, tmK, tmV, (ET*)out, rowmask, mask_words, meta,
+                                     q_pad, n_heads, n_kv_heads, n_splits, inv_sqrt_d, row_ml);
   if (e != cudaSuccess) { set_cuda_error(e, "cudaLaunchKernelEx(attn_fwd_tc_kernel)"); return LADE_ECUDA; }
   return LADE_OK;
+}
+
+template <typename ET>
+static int attn_fwd_tc_launch_t(cudaStream_t stream, const void* q, const void* k_cache, const void* v_cache, void* out,
+                                const uint32_t* rowmask, int mask_words, const int32_t* meta, void* scratch, int q_pad,
+                                int n_heads, int n_kv_heads, int head_dim, int kv_capacity, int kv_bound, int n_splits) {
+  (void)kv_bound;
+  if (head_dim != TC_D) return LADE_EUNSUPPORTED;
+  if (n_splits > 8) n_splits = 8;   // portable cluster size
+  return launch_tc<ET, false>(stream, q, k_cache, v_cache, out, rowmask, mask_words, meta, scratch, q_pad, n_heads,
+                              n_kv_heads, head_dim, kv_capacity, n_splits);
 }
 
 int attn_fwd_tc_launch(cudaStream_t stream, const void* q, const void* k_cache, const void* v_cache, void* out,
@@ -1015,56 +634,20 @@ int attn_fwd_tc_launch(cudaStream_t stream, const void* q, const void* k_cache, 
                                              n_heads, n_kv_heads, head_dim, kv_capacity, kv_bound, n_splits);
 }
 
-// impl 3: the reference-order variant.  kv_bound must bound kv_len + q_len of this call (the resident-S design holds at
-// most 3 KV tiles per split); the kernel traps if it does not.
+// impl 3: the reference-order variant.  kv_bound must bound kv_len + q_len of this call (every K/V tile of a split stays
+// resident in shared memory: at most 3 per split); the kernel traps if it does not.
 template <typename ET>
 static int attn_fwd_tc_exact_launch_t(cudaStream_t stream, const void* q, const void* k_cache, const void* v_cache, void* out,
                                       const uint32_t* rowmask, int mask_words, const int32_t* meta, void* scratch, int q_pad,
                                       int n_heads, int n_kv_heads, int head_dim, int kv_capacity, int kv_bound, int n_splits) {
   if (head_dim != TC_D) return LADE_EUNSUPPORTED;
-  const int q_tiles = (q_pad + TC_BM - 1) / TC_BM;
   if (n_splits > 8) n_splits = 8;
-  if (kv_bound < 1 || (kv_bound + TC_BN - 1) / TC_BN > 3 * n_splits) {
-    set_error_string("lade_attn_fwd impl 3: kv_bound exceeds 384 * n_splits (every S tile of a split must fit tensor memory)");
+  if (kv_bound < 1 || (kv_bound + TC_BN - 1) / TC_BN > TC_STAGES * n_splits) {
+    set_error_string("lade_attn_fwd impl 3: kv_bound exceeds 384 * n_splits (every K/V tile of a split must stay in shared memory)");
     return LADE_EUNSUPPORTED;
   }
-  if ((reinterpret_cast<uintptr_t>(q) & 15) || (reinterpret_cast<uintptr_t>(k_cache) & 15) ||
-      (reinterpret_cast<uintptr_t>(v_cache) & 15))
-    return LADE_EINVAL;
-  CUtensorMap tmQ, tmK, tmV;
-  int rc;
-  if ((rc = get_tensor_map(q, q_pad, n_heads, &tmQ)) != LADE_OK) return rc;
-  if ((rc = get_tensor_map(k_cache, kv_capacity, n_kv_heads, &tmK)) != LADE_OK) return rc;
-  if ((rc = get_tensor_map(v_cache, kv_capacity, n_kv_heads, &tmV)) != LADE_OK) return rc;
-  static unsigned long long attr_devs = 0;
-  int cur_dev = 0;
-  LADE_CUDA_CHECK(cudaGetDevice(&cur_dev));
-  if (!((attr_devs >> (cur_dev & 63)) & 1ull)) {
-    LADE_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_tc_exact_kernel<ET>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
-    attr_devs |= 1ull << (cur_dev & 63);
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(n_splits, n_heads, q_tiles);
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = TC_SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = n_splits;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  const float inv_sqrt_d = 1.0f / sqrtf((float)head_dim);
-  // the (max, sum) table of the rows lives where the L2 merge transport keeps its (m, l) pairs
-  float* part_o = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) + 65536);
-  float2* row_ml = reinterpret_cast<float2*>(part_o + (size_t)n_splits * n_heads * q_tiles * TC_BM * TC_D);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, attn_fwd_tc_exact_kernel<ET>, tmQ, tmK, tmV, (ET*)out, rowmask, mask_words, meta,
-                                     q_pad, n_heads, n_kv_heads, n_splits, inv_sqrt_d, row_ml);
-  if (e != cudaSuccess) { set_cuda_error(e, "cudaLaunchKernelEx(attn_fwd_tc_exact_kernel)"); return LADE_ECUDA; }
-  return LADE_OK;
+  return launch_tc<ET, true>(stream, q, k_cache, v_cache, out, rowmask, mask_words, meta, scratch, q_pad, n_heads,
+                             n_kv_heads, head_dim, kv_capacity, n_splits);
 }
 
 int attn_fwd_tc_exact_launch(cudaStream_t stream, const void* q, const void* k_cache, const void* v_cache, void* out,

@@ -1,6 +1,6 @@
-// Weight-streaming projection GEMM for the lookahead step on sm_100a (tcgen05 + TMA + TMEM).
+// Weight-streaming projection GEMM for the lookahead step on sm_90a (wgmma + TMA).
 //
-//   C[M, N] = A[M, K] · W[N, K]^T      bf16 in / bf16 out, fp32 accumulation in tensor memory
+//   C[M, N] = A[M, K] · W[N, K]^T      bf16 in / bf16 out, fp32 accumulation in registers
 //
 // Replaces the nn.Linear calls of the reference decoder layer on the lookahead step
 // (lade/models/modeling_llama.py:447-449 q/k/v_proj, :541 o_proj, :378 gate/up/down_proj, :1608 lm_head)
@@ -9,9 +9,9 @@
 //
 //   * one CTA per (N tile, K split); the tile width BN (32..256) and the K split (1/2/4/8) are picked per
 //     shape so that the CTA count lands just under the SM count (a single full wave);
-//   * warp 0 = TMA producer (A k-block [128 x 64] from L2, W k-block [BN x 64] from HBM, SWIZZLE_128B) into a
-//     4-8 stage mbarrier ring; warp 1 = tcgen05.mma issuer (M=128, N=BN, K=16 x 4 per k-block), accumulator
-//     [128 x BN] fp32 in TMEM; warps 2-5 = epilogue (tcgen05.ld -> bf16 -> global);
+//   * warp 8 = TMA producer (A k-block [128 x 64] from L2, W k-block [BN x 64] from HBM, SWIZZLE_128B) into a
+//     4-11 stage mbarrier ring; warps 0-7 = two consumer warpgroups, 64 rows of A each (the second one idles when
+//     M <= 64), wgmma m64n32k16 x BN / 32 per k16 step, accumulator [64 x BN] fp32 in registers;
 //   * K splits of one N tile form a thread-block cluster; their fp32 partial tiles are staged in shared memory
 //     and summed over distributed shared memory (no global scratch, no atomics, deterministic order).
 //
@@ -24,7 +24,8 @@
 
 namespace lade {
 
-constexpr int GM_THREADS = 192;
+constexpr int GM_THREADS = 288;          // two consumer warpgroups + one producer warp
+constexpr int GM_PRODUCER = 256;         // the producer thread
 constexpr int GM_BK = 64;                   // one SWIZZLE_128B atom of bf16 along K
 constexpr int GM_A_BYTES = 128 * GM_BK * 2; // 16 KB
 constexpr int GM_MAX_STAGES = 11;
@@ -96,24 +97,24 @@ __device__ __forceinline__ void reduce_splits(__nv_bfloat16* __restrict__ C, uin
 __global__ void __launch_bounds__(GM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
                __nv_bfloat16* __restrict__ C, int M, int N, int ldc, int kb_per_split, int BN, int stages, int split_k,
-               int prefill, uint32_t idesc, uint32_t tmem_cols, int launch_id) {
+               int prefill, int launch_id) {
   long long* tbuf = g_gemm_timing ? g_gemm_timing + 8ll * ((launch_id & 3) * 1024 + blockIdx.y * gridDim.x + blockIdx.x) : nullptr;
-  GM_STAMP(0, 0);
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // dynamic smem base is 1024-aligned by the launch (no static smem in this kernel)
-  // ring stage = [128 x 64] activations | [BN x 64] weights, one full / one empty mbarrier per stage
-  const uint32_t smem_base = smem_u32(smem_raw);
+  GM_STAMP(0, GM_PRODUCER);
+  extern __shared__ uint8_t smem_raw[];
+  // ring stage = [128 x 64] activations | [BN x 64] weights, one full / one empty mbarrier per stage; the base is
+  // aligned to 1024 bytes by hand (SWIZZLE_128B), the launch reserves the slack
+  const uint32_t raw_a = smem_u32(smem_raw);
+  const uint32_t smem_base = (raw_a + 1023u) & ~1023u;
+  uint8_t* smem = smem_raw + (smem_base - raw_a);
   const int stage_bytes = GM_A_BYTES + BN * 128;
   const uint32_t bars = smem_base + stages * stage_bytes;
-  uint8_t* bars_ptr = smem_raw + stages * stage_bytes;
   auto FULL = [&](int s) { return bars + 8u * s; };
   auto EMPTY = [&](int s) { return bars + 8u * (GM_MAX_STAGES + s); };
-  const uint32_t ACC_FULL = bars + 8u * (2 * GM_MAX_STAGES);
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(bars_ptr + 8 * (2 * GM_MAX_STAGES + 1));
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n0 = blockIdx.x * BN;
   const int kb0 = blockIdx.y * kb_per_split;
+  const int n_wg = M > 64 ? 2 : 1;                 // warpgroups with rows of A to multiply
 
   auto issue = [&](int kb) {
     const int s = kb % stages;
@@ -123,26 +124,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     tma_load_2d(sa, &tmA, FULL(s), (kb0 + kb) * GM_BK, 0);
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmW);
-      tma_prefetch_desc(&tmA);
-      for (int s = 0; s < stages; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 1); }
-      mbar_init(ACC_FULL, 1);
-      fence_barrier_init();
-      // nothing has to be waited for to fill the ring: do it before the CTA has finished setting up
-      if (prefill) for (int kb = 0; kb < stages; ++kb) issue(kb);
-    }
-    __syncwarp();
+  if (tid == GM_PRODUCER) {
+    tma_prefetch_desc(&tmW);
+    tma_prefetch_desc(&tmA);
+    for (int s = 0; s < stages; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 4 * n_wg); }
+    fence_barrier_init();
+    // nothing has to be waited for to fill the ring: do it before the CTA has finished setting up
+    if (prefill) for (int kb = 0; kb < stages; ++kb) issue(kb);
   }
-  if (warp == 1) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_slot;
-  GM_STAMP(1, 0);
+  GM_STAMP(1, GM_PRODUCER);
 
-  if (warp == 0) {
+  const int wg = warp >> 2;
+  const int g = lane >> 2, t = lane & 3;
+  const int row0 = wg * 64 + (warp & 3) * 16 + g;   // this thread's rows: row0 and row0 + 8
+  float acc[8][16];
+#pragma unroll
+  for (int c = 0; c < 8; ++c)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[c][i] = 0.f;
+
+  if (warp == 8) {
     if (lane == 0) {
       for (int kb = prefill ? stages : 0; kb < kb_per_split; ++kb) {
         if (kb >= stages) mbar_wait(EMPTY(kb % stages), ((kb / stages) - 1) & 1);
@@ -150,72 +152,65 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int kb = 0; kb < kb_per_split; ++kb) {
-        const int s = kb % stages;
-        mbar_wait(FULL(s), (kb / stages) & 1);
-        if (kb == 0) GM_STAMP(2, 32);
-        tc_fence_after();
-        const uint32_t sa = smem_base + s * stage_bytes;
+  } else if (wg < n_wg) {
+    for (int kb = 0; kb < kb_per_split; ++kb) {
+      const int s = kb % stages;
+      mbar_wait(FULL(s), (kb / stages) & 1);
+      if (kb == 0) GM_STAMP(2, 0);
+      const uint32_t sa = smem_base + s * stage_bytes;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t da = umma_desc(sa + k * 32, 16, 1024);
-          const uint64_t db = umma_desc(sa + GM_A_BYTES + k * 32, 16, 1024);
-          umma_bf16(tmem_acc, da, db, idesc, (kb | k) ? 1u : 0u);
-        }
-        umma_commit(EMPTY(s));
+      for (int c = 0; c < 8; ++c) wg_fence_regs(acc[c]);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint64_t da = wg_desc(sa + wg * 8192 + k * 32, 16, 1024);
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+          if (c * 32 < BN) wgmma_m64n32_ss_bf16(acc[c], da, wg_desc(sa + GM_A_BYTES + c * 4096 + k * 32, 16, 1024));
       }
-      umma_commit(ACC_FULL);
-      GM_STAMP(3, 32);
-    }
-    __syncwarp();
-  } else {
-    // epilogue warps 2..5: TMEM lane group = warp % 4
-    const int rg = warp & 3;
-    const int row = rg * 32 + lane;
-    mbar_wait(ACC_FULL, 0);
-    GM_STAMP(4, 64);
-    tc_fence_after();
-    const uint32_t taddr = tmem_acc + ((uint32_t)(rg * 32) << 16);
-    if (split_k == 1) {
-      __nv_bfloat16* crow = C + (size_t)row * ldc + n0;
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float v[32];
-        tmem_ld32(taddr + c0, v);
-        tmem_ld_wait();
-        if (row < M) {
+      wg_commit();
+      wg_wait_all();
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (n0 + c0 + j * 8 < N) {
-              uint4 o;
-              o.x = pack2_bf16(v[j * 8 + 0], v[j * 8 + 1]);
-              o.y = pack2_bf16(v[j * 8 + 2], v[j * 8 + 3]);
-              o.z = pack2_bf16(v[j * 8 + 4], v[j * 8 + 5]);
-              o.w = pack2_bf16(v[j * 8 + 6], v[j * 8 + 7]);
-              *reinterpret_cast<uint4*>(crow + c0 + j * 8) = o;
-            }
+      for (int c = 0; c < 8; ++c) wg_fence_regs(acc[c]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(EMPTY(s));
+    }
+    GM_STAMP(3, 0);
+    if (split_k == 1) {
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        if (c * 32 >= BN) continue;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int n = n0 + c * 32 + 8 * i;          // N % 8 == 0: a group of 8 columns is all in or all out
+          if (n >= N) continue;
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int r = row0 + 8 * rr;
+            if (r < M) *reinterpret_cast<uint32_t*>(C + (size_t)r * ldc + n + 2 * t) = pack2_bf16(acc[c][4 * i + 2 * rr], acc[c][4 * i + 2 * rr + 1]);
           }
         }
       }
-    } else {
-      // stage the fp32 partial tile over the (now idle) pipeline stages: row stride BN + 4 floats
-      float* s_acc = reinterpret_cast<float*>(smem_raw) + (size_t)row * (BN + 4);
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float v[32];
-        tmem_ld32(taddr + c0, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<float4*>(s_acc + c0 + j * 4) = make_float4(v[j * 4], v[j * 4 + 1], v[j * 4 + 2], v[j * 4 + 3]);
-      }
     }
-    GM_STAMP(5, 64);
   }
-  tc_fence_before();
-  __syncthreads();
+  GM_STAMP(4, 0);
 
   if (split_k > 1) {
+    __syncthreads();   // every warpgroup is done reading the stages before they are overwritten
+    if (warp < 8 && wg < n_wg) {
+      // stage the fp32 partial tile over the (now idle) pipeline stages: row stride BN + 4 floats
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        if (c * 32 >= BN) continue;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr)
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(smem) + (size_t)(row0 + 8 * rr) * (BN + 4) + c * 32 + 8 * i + 2 * t) =
+                make_float2(acc[c][4 * i + 2 * rr], acc[c][4 * i + 2 * rr + 1]);
+      }
+    }
+    GM_STAMP(5, 0);
     cluster_arrive();
     cluster_wait();
     GM_STAMP(6, 0);
@@ -226,7 +221,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     cluster_arrive();   // siblings may still be reading this CTA's partial tile
     cluster_wait();
   }
-  if (warp == 1) tmem_dealloc(tmem_acc, tmem_cols);
   GM_STAMP(7, 0);
 }
 
@@ -280,7 +274,7 @@ static int sm_count() {
   if (!n) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
@@ -369,9 +363,7 @@ int gemm_tc_launch(cudaStream_t stream, const void* a, const void* w, void* c, i
   if (stages > kbs) stages = kbs;
   if (stages < 1) return LADE_EINVAL;
   if (SK > 1 && 128 * (BN + 4) * 4 > stages * stage_bytes) return LADE_EINVAL;
-  const int smem = stages * stage_bytes + GM_BAR_BYTES;
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < BN) tmem_cols <<= 1;
+  const int smem = stages * stage_bytes + GM_BAR_BYTES + 1024;   // + slack to align the base to 1024 bytes
 
   CUtensorMap tmA, tmW;
   if ((rc = get_tensor_map_2d(a, a_rows, K, 128, false, &tmA)) != LADE_OK) return rc;
@@ -379,11 +371,10 @@ int gemm_tc_launch(cudaStream_t stream, const void* a, const void* w, void* c, i
   cudaLaunchConfig_t cfg;
   cudaLaunchAttribute attr[1];
   fill_launch_config(&cfg, attr, dim3((N + BN - 1) / BN, SK, 1), smem, SK, stream);
-  const uint32_t idesc = umma_idesc_n((uint32_t)BN, false);
   static int launch_counter = 0;
   const int prefill = (flags & 1) ? 0 : 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_tc_kernel, tmA, tmW, (__nv_bfloat16*)c, M, N, ldc, kbs, BN, stages, SK, prefill, idesc,
-                                     tmem_cols, launch_counter++);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_tc_kernel, tmA, tmW, (__nv_bfloat16*)c, M, N, ldc, kbs, BN, stages, SK, prefill,
+                                     launch_counter++);
   if (e != cudaSuccess) { set_cuda_error(e, "cudaLaunchKernelEx(gemm_tc_kernel)"); return LADE_ECUDA; }
   return LADE_OK;
 }

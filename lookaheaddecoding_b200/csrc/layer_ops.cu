@@ -202,7 +202,7 @@ __global__ void swiglu_kernel(const T* __restrict__ gate_up, T* __restrict__ out
 }
 
 // L2 prefetch of a weight range (fire-and-forget): one lane per CTA issues `cp.async.bulk.prefetch.L2` for chunks of
-// the range in a grid-stride loop and exits; the TMA engines pull the lines into the 126 MB L2 while OTHER kernels
+// the range in a grid-stride loop and exits; the TMA engines pull the lines into the 50 MB L2 while OTHER kernels
 // (attention, norms, RoPE -- phases of the step in which HBM is otherwise idle) run.  No data reaches the SM.
 __global__ void l2_prefetch_kernel(const char* __restrict__ base, long long bytes, int chunk) {
   // UBLKPF.L2 is a per-warp (uniform datapath) instruction: one lane per one-warp CTA issues, chunks interleaved over CTAs
@@ -293,7 +293,7 @@ static int swiglu_impl(void* stream, const void* gate_up, void* out, int32_t row
   if (!gate_up || !out || rows < 1 || inter < 8 || inter % 8 != 0) return LADE_EINVAL;
   const long long total = (long long)rows * (inter / 8);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   LADE_CUDA_CHECK(launch_pdl(swiglu_kernel<T>, dim3(blocks), dim3(256), 0, (cudaStream_t)stream,
                              (const T*)gate_up, (T*)out, rows, inter));
   return LADE_OK;

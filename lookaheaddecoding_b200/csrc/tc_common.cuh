@@ -1,8 +1,9 @@
-// Blackwell (sm_100a) PTX wrappers shared by the tcgen05 kernels: mbarrier, TMA, TMEM, tcgen05.mma, cluster / DSMEM.
+// Hopper (sm_90a) PTX wrappers shared by the tensor-core kernels: mbarrier, TMA, wgmma, cluster / DSMEM.
 #pragma once
 #include "common.cuh"
 
 #include <cuda.h>
+#include <type_traits>
 
 namespace lade {
 
@@ -37,8 +38,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
@@ -49,80 +48,67 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma (warpgroup MMA, sm_90a) ------------------------------------------------------------------------
+// Shared-memory matrix descriptor, SWIZZLE_128B (cute::GMMA::GmmaDescriptor):
+//   bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout = 1 (128-byte swizzle)
+// K-major operands: SBO = 1024 (next 8 rows), LBO unused.  MN-major operands: LBO = next 64-element block along M/N,
+// SBO = next 8 rows along K.
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int N>
+__device__ __forceinline__ void wg_fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-  const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]) : "memory");
-}
-__device__ __forceinline__ float tmem_ld1(uint32_t taddr) {         // one 32-bit column of this thread's lane
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-  return __uint_as_float(r);
-}
-__device__ __forceinline__ void tmem_st1(uint32_t taddr, float v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(__float_as_uint(v)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory descriptor (cute::UMMA::SmemDescriptor, version 1, SWIZZLE_128B):
-//   bits [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
+#define LADE_WG_O4(d, i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define LADE_WG_O16(d, i) LADE_WG_O4(d, i), LADE_WG_O4(d, i + 4), LADE_WG_O4(d, i + 8), LADE_WG_O4(d, i + 12)
+#define LADE_WG_O64(d) LADE_WG_O16(d, 0), LADE_WG_O16(d, 16), LADE_WG_O16(d, 32), LADE_WG_O16(d, 48)
+#define LADE_WG_R64 \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, " \
+  "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+
+// D[64 x 128] (+)= A[64 x 16] . B[16 x 128]; A and B from shared memory, both K-major; fp32 accumulators.
+template <typename ET>
+__device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (std::is_same<ET, __half>::value) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " LADE_WG_R64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : LADE_WG_O64(d) : "l"(da), "l"(db), "r"(accumulate));
+  } else {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " LADE_WG_R64 ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+                 : LADE_WG_O64(d) : "l"(da), "l"(db), "r"(accumulate));
+  }
 }
-// Same descriptor without swizzling (layout type 0): core matrices of 8 rows x 16 bytes at strides LBO / SBO.
-__device__ __forceinline__ uint64_t umma_desc_noswizzle(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
+// D[64 x 128] += A[64 x 16] . B[16 x 128]; A from registers (the m64k16 fragment: 4 packed pairs per thread), B from
+// shared memory, MN-major (transposed).
+template <typename ET>
+__device__ __forceinline__ void wgmma_m64n128_rs_tb(float (&d)[64], const uint32_t* a, uint64_t db) {
+  if constexpr (std::is_same<ET, __half>::value) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " LADE_WG_R64 ", {%64, %65, %66, %67}, %68, 1, 1, 1, 1;"
+                 : LADE_WG_O64(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+  } else {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " LADE_WG_R64 ", {%64, %65, %66, %67}, %68, 1, 1, 1, 1;"
+                 : LADE_WG_O64(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+  }
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): f32 accumulate, bf16 x bf16, M=128, N = n (multiple of 16).
-__host__ __device__ constexpr uint32_t umma_idesc_n(uint32_t n, bool b_mn_major, bool fp16_operands = false) {
-  // bits [7,10) = A format, [10,13) = B format: 0 = F16, 1 = BF16 (kind::f16)
-  return (1u << 4) | ((fp16_operands ? 0u : 1u) << 7) | ((fp16_operands ? 0u : 1u) << 10) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((n >> 3) << 17) | ((128u >> 4) << 24);
+// D[64 x 32] += A[64 x 16] . B[16 x 32], bf16, both K-major from shared memory.
+__device__ __forceinline__ void wgmma_m64n32_ss_bf16(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, 1, 1, 1, 0, 0;"
+               : LADE_WG_O16(d, 0) : "l"(da), "l"(db));
 }
 
 __device__ __forceinline__ float ex2_approx(float x) {

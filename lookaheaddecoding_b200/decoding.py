@@ -142,7 +142,7 @@ def jacobi_greedy_search_multilevel(self, input_ids: torch.LongTensor, logits_pr
                                     output_hidden_states=None, output_scores=None,
                                     return_dict_in_generate=None, synced_gpus: bool = False, streamer=None,
                                     chat: bool = False, stop_token: Optional[str] = None, **model_kwargs):
-    """Greedy lookahead decoding on the B200 engine; drop-in for lade/decoding.py:697-1259.
+    """Greedy lookahead decoding on the H100 engine; drop-in for lade/decoding.py:697-1259.
 
     Inherited restrictions (fail loudly, as the reference asserts): batch size 1
     (modeling_llama.py:1448), no logits processors (:968), ``return_dict_in_generate == False``

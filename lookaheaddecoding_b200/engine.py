@@ -1,4 +1,4 @@
-"""Host-side driver of the B200 lookahead/verification step.
+"""Host-side driver of the H100 lookahead/verification step.
 
 One ``LookaheadEngine`` wraps one HF ``LlamaForCausalLM`` on one GPU.  Per decoding step it launches
 (through the C-ABI of ``include/lade_sm100.h``):
@@ -8,7 +8,7 @@ One ``LookaheadEngine`` wraps one HF ``LlamaForCausalLM`` on one GPU.  Per decod
     -> lade_rmsnorm_gather (live lm_head rows only) -> lm_head GEMM -> lade_argmax_rows ->
     lade_accept_update -> lade_kv_compact
 
-which is the B200 re-design of one iteration of the reference's ``while True`` loop
+which is the GPU re-design of one iteration of the reference's ``while True`` loop
 (``lade/decoding.py:923-1219``) including ``jforward_multilevel``
 (``lade/models/modeling_llama.py:1381-1608``).  The dense projections are plain library GEMMs
 (cuBLAS through ``torch.mm``); everything else is this repo's CUDA.  All per-step scalars live in
@@ -57,9 +57,8 @@ class LookaheadEngine:
                  prefetch_ctas: int = 32, prefetch_chunk: int = 32768):
         self.lib = _cabi.load()
         # L2 weight prefetch on a side branch of the step graph (see _prefetch): MB of the NEXT projection's weights
-        # requested while [rmsnorm | rope+attention | rmsnorm | swiglu | final norm] run.  MEASURED NEGATIVE on B200
-        # (profiles/r02_l2_prefetch_ab.md: 254 -> 232 tokens/s with 32/110/32/36/36 MB, 246 with the attention window
-        # only; a projection reading L2-resident weights is only 10-15 % faster than from HBM): OFF unless asked for.
+        # requested while [rmsnorm | rope+attention | rmsnorm | swiglu | final norm] run.  OFF unless asked for: the
+        # H100's 50 MB L2 holds little of one projection's weights, and no gain has been measured there.
         import os as _os
         if l2_prefetch is None:
             l2_prefetch = _os.environ.get("LADE_L2_PREFETCH", "0") == "1"
@@ -142,7 +141,7 @@ class LookaheadEngine:
         self.rec_ints = int(self.lib.lade_lp_record_ints(C.byref(probe)))
         sm = torch.cuda.get_device_properties(self.dev).multi_processor_count
         q_tiles = (self.q_steady + 127) // 128
-        # one CTA per SM (TMEM/smem bound): keep the split grid within a single wave
+        # one CTA per SM (shared-memory bound): keep the split grid within a single wave
         self.attn_splits = int(attn_splits) if attn_splits else max(1, min(8, sm // (self.nh * q_tiles)))   # <= 8: the splits of a head form a thread-block cluster
 
         # non-prefill steps: the steady shape, or a window-fill step when it is larger (G = 0 and W < N-2 ...)
@@ -150,7 +149,7 @@ class LookaheadEngine:
                                                    for k in range(1, self.N - 1)])
         self.kv_capacity = self.max_total_len + self.q_nonprefill + self.WCAP + 8
         # kv_bound of lade_attn_fwd: an upper bound of kv_len + q_len over the whole generation.  Only impl 3 (the
-        # reference-order variant, every S tile of a split resident in tensor memory) needs a tight one: at most
+        # reference-order variant, every K/V tile of a split resident in shared memory) needs a tight one: at most
         # 3 KV tiles of 128 rows per split and 8 splits per head
         self.attn_kv_bound = self.kv_capacity
         if self.attn_impl == 3:

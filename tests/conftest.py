@@ -10,8 +10,8 @@ for _p in (ROOT, os.path.dirname(os.path.abspath(__file__))):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
-    config.addinivalue_line("markers", "reference: needs the unmodified reference at /root/reference")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
+    config.addinivalue_line("markers", "reference: needs the unmodified reference (baseline/ref_loader.py)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -13,7 +13,7 @@ either difference removed through the engine's checker hooks:
   B  projections issued call for call like the reference (engine._unfused_gemms)
   C  attention replaced by the restated reference math in torch on the engine's own Q / KV cache (engine._attn_hook)
   D  B + C
-  E  the engine with attn_impl=3: the tcgen05 kernel's reference-order variant (no hooks, CUDA graph on)
+  E  the engine with attn_impl=3: the wgmma kernel's reference-order variant (no hooks, CUDA graph on)
 
 and prints one JSON line with the number of divergences of each against the reference's own self-inconsistency on the
 same run (ids of its lookahead loop vs its own teacher-forced forward).  usage (GPU box):
@@ -75,7 +75,7 @@ def main():
     out = {"compared_tokens": args.max_new, "prompt_len": P,
            "reference_self_mismatches": self_rep["n_self_mismatch"], "modes": {}}
     names = {"A": "as shipped", "B": "projections call for call", "C": "reference-order attention (torch)",
-             "D": "both", "E": "attn_impl=3 (reference-order tcgen05 kernel)"}
+             "D": "both", "E": "attn_impl=3 (reference-order wgmma kernel)"}
     for mode in args.modes.split(","):
         eng = LookaheadEngine(model, W, N, G, pool_from_prompt=True, max_total_len=P + args.max_new + 8,
                               use_cuda_graph=mode in ("A", "B", "E"), attn_impl=3 if mode == "E" else 0)

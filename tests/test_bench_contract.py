@@ -1,6 +1,5 @@
-"""bench.py's reference arm (the UNMODIFIED reference from baseline/_ref on the host cores) honours the driver's JSON
-contract.  Run on the tiny workload so that the CPU suite stays fast; the 7B line is the same code path."""
-import json
+"""bench.py's reference arm (the UNMODIFIED reference from baseline/_ref on the host cores) under lookahead parallelism:
+only rank 0 prints a result line.  Run on the tiny workload so that the CPU suite stays fast."""
 import os
 import subprocess
 import sys
@@ -13,24 +12,6 @@ def _run(extra_env=None, args=()):
     env.update(extra_env or {})
     return subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--workload", "tiny", *args],
                           capture_output=True, text=True, env=env, timeout=600, cwd=ROOT)
-
-
-def test_reference_arm_prints_one_contract_line():
-    res = _run(args=("--steps", "2", "--warmup", "1"))
-    assert res.returncode == 0, res.stderr[-2000:]
-    lines = [l for l in res.stdout.splitlines() if l.startswith("{")]
-    assert len(lines) == 1
-    d = json.loads(lines[0])
-    for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "higher_is_better", "scaling", "vs_baseline", "dtype",
-                "data", "config", "impl", "cpu_baseline", "e2e", "gpu_launches"):
-        assert key in d, key
-    assert d["impl"] == "reference" and d["unit"] == "tokens/s" and d["higher_is_better"] is True
-    assert d["vs_baseline"] is None and d["gpu_launches"] == 0 and "workload" in d["config"]
-    cb = d["cpu_baseline"]
-    assert cb["kind"] == "reference" and cb["cores"] >= 1 and cb["value"] == d["value"] and cb["value"] > 0
-    assert cb["steady_steps_timed"] >= 2 and cb["s_per_steady_step"] > 0 and "UNMODIFIED reference" in cb["sample"]
-    assert d["ms_per_step"] == round(1e3 * cb["s_per_steady_step"], 1)
-    assert d["e2e"] == {"value": d["value"], "unit": "tokens/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
 
 
 def test_reference_arm_other_ranks_exit_silently():

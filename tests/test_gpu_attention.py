@@ -16,7 +16,7 @@ from oracle import lookahead as LA
 
 pytestmark = pytest.mark.gpu
 ATOL_MAX, ATOL_MEAN = 2e-2, 2e-3
-IMPLS = [int(x) for x in os.environ.get("LADE_TEST_ATTN_IMPLS", "2,1").split(",")]   # 2 = tcgen05 (product default), 1 = mma.sync fallback
+IMPLS = [int(x) for x in os.environ.get("LADE_TEST_ATTN_IMPLS", "2,1").split(",")]   # 2 = wgmma/TMA (product default), 1 = mma.sync
 
 
 def run_kernel(q, k, v, lay, meta_vals, q_pad, n_splits, impl, kv_capacity=None, dt=torch.bfloat16):
@@ -104,8 +104,7 @@ def _oracle_attn(q, k, v, lay, kv_len):
     (0, 15, 5, 15, 2, 2, 1), (1, 15, 5, 15, 2, 2, 2), (63, 15, 5, 3, 4, 2, 2), (64, 15, 5, 15, 2, 2, 5),
     (1000, 15, 5, 15, 8, 8, 5), (3001, 15, 5, 0, 4, 4, 7), (517, 20, 7, 20, 4, 4, 3), (200, 5, 3, 3, 2, 1, 4),
     (130, 60, 8, 7, 2, 2, 2),
-    # more than 4 KV tiles per split: the 3-deep ring whose merge slots alias the K/V stages (shorter launches run
-    # the 2-deep ring with dedicated slots)
+    # more than 3 KV tiles per split: the K/V ring wraps around
     (3001, 15, 5, 15, 2, 2, 3), (2300, 15, 5, 15, 4, 2, 4),
 ])
 def test_attention_steady_shapes_vs_oracle(kv_len, W, N, g, Hq, Hkv, splits, impl):
@@ -156,7 +155,7 @@ def test_attention_lp_shapes_vs_oracle(impl):
 
 @pytest.mark.parametrize("kv_len,Hq,Hkv,splits", [(0, 4, 4, 1), (77, 4, 2, 3), (700, 8, 2, 4)])
 def test_attention_head_dim_64_vs_oracle(kv_len, Hq, Hkv, splits):
-    """head_dim 64 (TinyLlama-style): served by the mma.sync kernel (impl 0 picks it; the tcgen05 kernel is 128-only)."""
+    """head_dim 64 (TinyLlama-style): served by the mma.sync kernel (impl 0 picks it; the wgmma kernel is 128-only)."""
     torch.manual_seed(kv_len + 64)
     W, N, g = 15, 5, 7
     gs = N - 1
@@ -175,12 +174,12 @@ def test_attention_head_dim_64_vs_oracle(kv_len, Hq, Hkv, splits):
     z = torch.zeros(64, device="cuda")
     rc = lib.lade_attn_fwd(0, z.data_ptr(), z.data_ptr(), z.data_ptr(), z.data_ptr(), 0, 0, z.data_ptr(), z.data_ptr(), 8, 2, 2, 64,
                            16, 16, 1, 2)
-    assert rc == _cabi.LADE_EUNSUPPORTED          # the tcgen05 kernel refuses head_dim 64 when forced
+    assert rc == _cabi.LADE_EUNSUPPORTED          # the wgmma kernel refuses head_dim 64 when forced
 
 
 @pytest.mark.parametrize("kv_len,D,Hq,Hkv,splits", [(0, 128, 2, 2, 1), (300, 128, 4, 2, 3), (130, 64, 4, 2, 2)])
 def test_attention_fp16_vs_oracle(kv_len, D, Hq, Hkv, splits):
-    """fp16 models: lade_attn_fwd_f16 (impl 0: tcgen05 kernel on fp16 operands for head_dim 128, mma.sync for 64; impl 1:
+    """fp16 models: lade_attn_fwd_f16 (impl 0: wgmma kernel on fp16 operands for head_dim 128, mma.sync for 64; impl 1:
     mma.sync) against the reference's eager attention restated in fp16; same absolute tolerance as bf16."""
     torch.manual_seed(kv_len + D)
     W, N, g = 15, 5, 5
@@ -201,7 +200,7 @@ def test_attention_fp16_vs_oracle(kv_len, D, Hq, Hkv, splits):
         check_close(out, want)
 
 
-# ---- impl 3: the tcgen05 kernel's reference-order variant (probabilities normalised BEFORE they are rounded) ----------
+# ---- impl 3: the wgmma kernel's reference-order variant (probabilities normalised BEFORE they are rounded) ----------
 def _mismatch(a, b):
     return (a != b).float().mean().item()
 
@@ -281,7 +280,7 @@ def test_reference_order_variant_fp16_and_bounds():
     out = run_kernel(q, k, v, lay, meta_for(lay, kv_len, q_pad), q_pad, 3, 3, dt=torch.float16)
     check_close(out, want)
     assert _mismatch(out, want) <= 0.02
-    # more than 3 KV tiles per split do not fit tensor memory: refused on the host, loudly (T = 480 rows on one split)
+    # more than 3 KV tiles per split do not fit shared memory: refused on the host, loudly (T = 480 rows on one split)
     k2 = torch.randn(Hkv, 400 + q_len, 128, device="cuda").to(torch.float16)
     with pytest.raises(Exception):
         run_kernel(q, k2, k2, lay, meta_for(lay, 400, q_pad), q_pad, 1, 3, dt=torch.float16)

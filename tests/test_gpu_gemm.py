@@ -1,4 +1,4 @@
-"""tcgen05 weight-streaming projection GEMM (lade_gemm_bf16) vs torch: C = A . W^T, bf16 in/out, fp32 accumulate.
+"""wgmma weight-streaming projection GEMM (lade_gemm_bf16) vs torch: C = A . W^T, bf16 in/out, fp32 accumulate.
 
 The reference computes these with nn.Linear (modeling_llama.py:447-449,541,378,1608).  Accumulation order differs
 from cuBLAS, so results may differ by one bf16 ulp on a small fraction of elements; the test bounds both the

@@ -1,5 +1,7 @@
-"""GPU-vs-GPU token-id parity: this repo's engine against the UNMODIFIED reference (baseline/_ref) run on the same B200
-with the same weight tensors (baseline/parity.py).
+"""GPU-vs-GPU token-id parity: this repo's engine against the UNMODIFIED reference run on an H100 with the same weight
+tensors (baseline/parity.py).  The reference's side -- its ids and its model's next-token logits at every position -- is
+recorded in tests/golden/parity_ref.json.gz by tests/golden/gen_golden_parity.py; the weights are rebuilt here from the
+same device seed (bench.build_model).
 
 BASELINE.json config 1 (tiny random-init Llama, W5 N3 G3 -- with head_dim 128 so the production kernel runs), the
 7B-config lookahead shape W15 N5 G15 on the tiny model, and the edge shapes of tests/golden/greedy_edge_traces.json.gz
@@ -9,16 +11,19 @@ through the ENGINE (the state-machine replay of those traces is in test_gpu_stat
 Pass criterion: ids identical, or every divergence is a near-tie on the reference model's own logits (<= 3 bf16 ulps
 below its top logit for both candidates); every position is compared (the reference's token is forced after a
 divergence).  The report is printed (run with -s) and the exact cases are asserted exact."""
+import functools
+import gzip
+import json
+import os
 import random
 
 import pytest
 import torch
 
 from baseline import parity as PAR
-from baseline import ref_loader as R
+from helpers import GOLD
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(not R.reference_available(), reason="unmodified reference not present (baseline/_ref)")]
+pytestmark = pytest.mark.gpu
 
 TINY = dict(hidden=256, layers=2, heads=2, kv_heads=2, inter=688, vocab=32000, max_pos=2048, rope_theta=10000.0, eps=1e-5)
 GQA = dict(hidden=512, layers=2, heads=4, kv_heads=2, inter=688, vocab=4096, max_pos=2048, rope_theta=10000.0, eps=1e-5)
@@ -44,14 +49,32 @@ CASES = [("cfg1_w5n3g3",       TINY, 5,  3, 3,  64, 96, False),
          ("edge_w2n4g1",       TINY, 2,  4, 1,  16, 32, True),
          ("edge_g1_w15n5",     TINY, 15, 5, 1,  32, 48, True),
          ("edge_n3_w20g20",    TINY, 20, 3, 20, 24, 48, True)]
+FP16_CASES = ("cfg1_w5n3g3_pool", "w15n5g15", "gqa_w15n5g15", "d64_gqa_w15n5g15", "edge_p1")
 
 
-def build_pair(shape, seed=0, dtype=torch.bfloat16):
+def build_hf(shape, seed=0, dtype=torch.bfloat16):
     from bench import build_model
     hf = build_model(shape, torch.device("cuda"), seed=seed)
     if dtype != torch.bfloat16:
         hf = hf.to(dtype)
+    return hf
+
+
+def build_pair(shape, seed=0, dtype=torch.bfloat16):
+    """The HF model and the unmodified reference model sharing its weights (recording the golden data only)."""
+    hf = build_hf(shape, seed, dtype)
     return hf, PAR.reference_model_sharing_weights(hf, shape)
+
+
+@functools.lru_cache(maxsize=1)
+def _gold():
+    with gzip.open(os.path.join(GOLD, "parity_ref.json.gz"), "rt") as f:
+        return json.load(f)
+
+
+def stored(key, dtype=torch.bfloat16):
+    """The recorded reference run `key` (see tests/golden/gen_golden_parity.py)."""
+    return PAR.StoredReference(_gold()[key], 10 if dtype == torch.float16 else 7)
 
 
 def engine_generate(hf, W, N, G, pool, cap, eos=(), **engine_kw):
@@ -65,11 +88,11 @@ def engine_generate(hf, W, N, G, pool, cap, eos=(), **engine_kw):
 
 @pytest.mark.parametrize("name,shape,W,N,G,P,new,pool", CASES, ids=[c[0] for c in CASES])
 def test_engine_ids_match_reference_on_the_same_gpu(name, shape, W, N, G, P, new, pool):
-    hf, ref = build_pair(shape)
+    hf, ref = build_hf(shape), stored(name)
     g = torch.Generator().manual_seed(1)
     prompt = torch.randint(3, shape["vocab"], (P,), generator=g).tolist()
-    ref_ids, ref_steps = PAR.reference_greedy(ref, prompt, new, W, N, G, py_seed=0, pool_from_prompt=pool)
-    assert len(ref_ids) == P + new
+    ref_ids, ref_steps = ref.ids, ref.steps
+    assert ref_ids[:P] == prompt and len(ref_ids) == P + new
     eng, gen = engine_generate(hf, W, N, G, pool, P + new)
     rep = PAR.compare_ids(gen, ref_ids, P, ref)
     print(f"\n{name}: exact={rep['exact']} exact_prefix={rep['exact_prefix_tokens']}/{rep['compared_tokens']} "
@@ -80,12 +103,11 @@ def test_engine_ids_match_reference_on_the_same_gpu(name, shape, W, N, G, P, new
 
 
 def test_eos_on_first_token_matches_reference():
-    hf, ref = build_pair(TINY)
+    hf, ref = build_hf(TINY), stored("eos_first_token")
     g = torch.Generator().manual_seed(1)
     prompt = torch.randint(3, 32000, (12,), generator=g).tolist()
-    free, _ = PAR.reference_greedy(ref, prompt, 16, 5, 3, 3, py_seed=0, pool_from_prompt=True)
-    eos = free[12]
-    ref_ids, _ = PAR.reference_greedy(ref, prompt, 16, 5, 3, 3, py_seed=0, eos_token_id=[eos], pool_from_prompt=True)
+    eos = ref.rec["eos"]                       # the reference's first free-running token
+    ref_ids = ref.ids
     assert ref_ids == prompt + [eos]
     eng, gen = engine_generate(hf, 5, 3, 3, True, 12 + 16, eos=[eos])
     ours = gen(prompt, 16)
@@ -100,12 +122,11 @@ def test_window_fill_step_larger_than_steady_and_host_stopping_criteria():
     silent clamp); output == the reference model's plain greedy.  Then a custom StoppingCriteria through generate()."""
     import lade
     from transformers import StoppingCriteria, StoppingCriteriaList
-    hf, ref = build_pair(TINY)
+    hf, ref = build_hf(TINY), stored("plain_greedy_p10")
     g = torch.Generator().manual_seed(3)
     prompt = torch.randint(3, 32000, (10,), generator=g).tolist()
-    ar = list(prompt)
-    for _ in range(24):
-        ar.append(int(torch.argmax(PAR.reference_next_logits(ref, ar))))
+    ar = ref.ids                               # the reference model's plain greedy: argmax of its causal forward
+    assert ar[:10] == prompt and len(ar) == 10 + 24
     eng, gen = engine_generate(hf, 5, 8, 0, False, 10 + 24)
     assert eng.q_nonprefill > eng.q_steady
     rep = PAR.compare_ids(gen, ar, 10, ref)
@@ -135,17 +156,17 @@ def test_window_fill_step_larger_than_steady_and_host_stopping_criteria():
         os.environ["USE_LADE"] = "0"
 
 
-@pytest.mark.parametrize("name,shape,W,N,G,P,new,pool", [c for c in CASES if c[0] in ("cfg1_w5n3g3_pool", "w15n5g15", "gqa_w15n5g15",
-                                                                                     "d64_gqa_w15n5g15", "edge_p1")],
+@pytest.mark.parametrize("name,shape,W,N,G,P,new,pool", [c for c in CASES if c[0] in FP16_CASES],
                          ids=lambda v: v if isinstance(v, str) else None)
 def test_fp16_engine_ids_match_reference_on_the_same_gpu(name, shape, W, N, G, P, new, pool):
     """fp16 models (the dtype of the reference's README / minimal.py): the *_f16 kernels against the unmodified reference
     running in fp16 on the same GPU and weights; ties are measured in fp16 ulps."""
-    hf, ref = build_pair(shape, dtype=torch.float16)
-    assert next(ref.parameters()).dtype == torch.float16
+    hf, ref = build_hf(shape, dtype=torch.float16), stored(name + "_fp16", torch.float16)
+    assert next(hf.parameters()).dtype == torch.float16
     g = torch.Generator().manual_seed(1)
     prompt = torch.randint(3, shape["vocab"], (P,), generator=g).tolist()
-    ref_ids, ref_steps = PAR.reference_greedy(ref, prompt, new, W, N, G, py_seed=0, pool_from_prompt=pool)
+    ref_ids, ref_steps = ref.ids, ref.steps
+    assert ref_ids[:P] == prompt
     eng, gen = engine_generate(hf, W, N, G, pool, P + new)
     assert eng.dt == torch.float16
     rep = PAR.compare_ids(gen, ref_ids, P, ref)
@@ -163,10 +184,11 @@ def test_fp16_engine_ids_match_reference_on_the_same_gpu(name, shape, W, N, G, P
                          ids=["w15n5g15_pool", "w20n7g20_pool", "gqa_w15n5g15", "edge_p1"])
 def test_reference_order_attention_engine_ids(name, shape, W, N, G, P, new, pool):
     """attn_impl=3: the attention variant that rounds the probabilities like the reference, through the whole engine."""
-    hf, ref = build_pair(shape)
+    hf, ref = build_hf(shape), stored(name)
     g = torch.Generator().manual_seed(1)
     prompt = torch.randint(3, shape["vocab"], (P,), generator=g).tolist()
-    ref_ids, _ = PAR.reference_greedy(ref, prompt, new, W, N, G, py_seed=0, pool_from_prompt=pool)
+    ref_ids = ref.ids
+    assert ref_ids[:P] == prompt
     eng, gen = engine_generate(hf, W, N, G, pool, P + new, attn_impl=3)
     rep = PAR.compare_ids(gen, ref_ids, P, ref)
     print(f"\n{name} (attn_impl=3): exact={rep['exact']} divergences={rep['n_divergences']}")
@@ -175,7 +197,7 @@ def test_reference_order_attention_engine_ids(name, shape, W, N, G, P, new, pool
 
 
 def test_reference_order_attention_refuses_contexts_it_cannot_hold():
-    """attn_impl=3 keeps every S tile of a split in tensor memory: more than 3072 rows of context (3 tiles x 8 splits)
+    """attn_impl=3 keeps every K/V tile of a split in shared memory: more than 3072 rows of context (3 tiles x 8 splits)
     are refused when the engine is built, never silently downgraded."""
     from bench import build_model
     from lookaheaddecoding_b200 import LookaheadEngine

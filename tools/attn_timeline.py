@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-CTA phase timeline of the tcgen05 attention kernel (lade_debug_attn_timing)."""
+"""Per-CTA phase timeline of the wgmma attention kernel (lade_debug_attn_timing)."""
 import os, sys, json
 import numpy as np
 import torch

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-CTA phase timeline of the tcgen05 projection GEMM (lade_debug_gemm_timing, %globaltimer ns).
+"""Per-CTA phase timeline of the wgmma projection GEMM (lade_debug_gemm_timing, %globaltimer ns).
 
 Four back-to-back launches on distinct weights are replayed from a CUDA graph; for each launch the phases are
 reported relative to the earliest CTA start of that launch, plus the idle gap to the previous launch's last exit.

@@ -2,7 +2,7 @@
 """Per-kernel totals and shares of an `ncu --metrics gpu__time_duration.sum --csv` launch list (cold-cache, serialised
 launches: compare SHARES with the in-graph ablation, never the absolute times).
 
-  python tools/launch_shares.py profiles/r02_launches_steady.csv [--top 20]
+  python tools/launch_shares.py launches.csv [--top 20]
 """
 import argparse
 import collections

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Pull the judged metrics of one kernel launch out of .ncu-rep captures into a small JSON (profiles/*_ncu_summary.json).
+"""Pull the judged metrics of one kernel launch out of .ncu-rep captures into a small JSON.
 
 usage: ncu_extract.py label=path.ncu-rep [label=path.ncu-rep ...] > summary.json     (takes the LAST captured launch)"""
 import csv, io, json, subprocess, sys

@@ -3,8 +3,7 @@
 #   tools/run_sanitizer.sh <tool: memcheck|racecheck|synccheck|initcheck> <log> [pytest node ids...]
 # Round-1 lesson: the first `import torch` on a fresh box takes ~1 min, longer than the sanitizer's default launch
 # time-out ("No attachable process found") -> page the image in first and raise --launch-timeout.
-# Round-2 lesson: the pass over the kernels BEFORE programmatic dependent launch was extended (profiles/
-# r02_sanitizer_*.log) is clean; a second pass over the final kernels -- every glue kernel launched with the programmatic
+# Round-2 lesson: the pass over the kernels BEFORE programmatic dependent launch was extended is clean; a second pass over the final kernels -- every glue kernel launched with the programmatic
 # attribute, griddepcontrol in the attention kernel, st.shared::cluster merge, Philox sampling kernel -- took the GPU box
 # down twice (box lost ~3 min into memcheck, nothing returned).  The runner therefore switches PDL off; do not point it
 # at PDL launches on a shared box.
