@@ -203,13 +203,6 @@ int lade_debug_gemm_timing(void* dev_buffer);
 /* act = bf16(silu(gate)) * up on the fused [rows][2*inter] projection.  LlamaMLP, modeling_llama.py:378. */
 int lade_swiglu(void* stream, const void* gate_up, void* out, int32_t rows, int32_t inter);
 
-/* Fire-and-forget prefetch of [ptr, ptr + bytes) into the L2 (cp.async.bulk.prefetch.L2, `chunk_bytes` per request,
- * `n_ctas` one-warp CTAs).  No reference counterpart: the reference streams every projection weight from DRAM when its
- * F.linear runs (modeling_llama.py:447-449,:378,:541).  Here the host queues the prefetch of the NEXT projection's
- * weights on a side branch of the step graph, parallel to the attention / norm / RoPE kernels, whose phases leave
- * HBM idle; the projection then finds (part of) its weights in the 50 MB L2.  ptr 16-byte aligned. */
-int lade_l2_prefetch(void* stream, const void* ptr, int64_t bytes, int32_t n_ctas, int32_t chunk_bytes);
-
 /* fp16 models (the dtype of the reference's README.md:159 / minimal.py:19; the BASELINE configs are bf16): the same
  * kernels instantiated on the element type -- every rounding point of the bf16 entry point of the same name without the
  * suffix happens in fp16 instead.  Arguments, layouts and error codes are those of the unsuffixed function.

@@ -51,7 +51,6 @@ _SIGNATURES = {
     "lade_gemm_bf16": (C.c_int, [c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
     "lade_debug_gemm_timing": (C.c_int, [c_p]),
     "lade_swiglu": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32]),
-    "lade_l2_prefetch": (C.c_int, [c_p, c_p, C.c_int64, c_i32, c_i32]),
     "lade_argmax_rows": (C.c_int, [c_p, c_p, c_i32, c_i32, c_i32, c_p]),
     "lade_accept_update": (C.c_int, [c_p, c_p, c_p, c_p, c_p]),
     "lade_commit_decision": (C.c_int, [c_p, c_p, c_p, c_p, c_p]),

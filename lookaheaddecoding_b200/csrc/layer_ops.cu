@@ -201,23 +201,6 @@ __global__ void swiglu_kernel(const T* __restrict__ gate_up, T* __restrict__ out
   }
 }
 
-// L2 prefetch of a weight range (fire-and-forget): one lane per CTA issues `cp.async.bulk.prefetch.L2` for chunks of
-// the range in a grid-stride loop and exits; the TMA engines pull the lines into the 50 MB L2 while OTHER kernels
-// (attention, norms, RoPE -- phases of the step in which HBM is otherwise idle) run.  No data reaches the SM.
-__global__ void l2_prefetch_kernel(const char* __restrict__ base, long long bytes, int chunk) {
-  // UBLKPF.L2 is a per-warp (uniform datapath) instruction: one lane per one-warp CTA issues, chunks interleaved over CTAs
-  if (threadIdx.x != 0) return;
-  const long long n_chunks = (bytes + chunk - 1) / chunk;
-  for (long long i = blockIdx.x; i < n_chunks; i += gridDim.x) {
-    const long long off = i * chunk;
-    long long sz = bytes - off;
-    if (sz > chunk) sz = chunk;
-    sz &= ~15ll;                                           // size operand: multiple of 16 bytes
-    if (sz > 0)
-      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(base + off), "r"((unsigned)sz) : "memory");
-  }
-}
-
 }  // namespace lade
 
 using namespace lade;
@@ -227,15 +210,6 @@ extern "C" {
 static int norm_threads(int hidden) {
   int t = ((hidden / 8 + 31) / 32) * 32;
   return t < 128 ? 128 : (t > 1024 ? 1024 : t);
-}
-
-int lade_l2_prefetch(void* stream, const void* ptr, int64_t bytes, int32_t n_ctas, int32_t chunk_bytes) {
-  if (!ptr || bytes < 0 || n_ctas < 1 || chunk_bytes < 16 || (chunk_bytes & 15) || (reinterpret_cast<uintptr_t>(ptr) & 15))
-    return LADE_EINVAL;
-  if (bytes == 0) return LADE_OK;
-  l2_prefetch_kernel<<<n_ctas, 32, 0, (cudaStream_t)stream>>>((const char*)ptr, bytes, chunk_bytes);
-  LADE_LAUNCH_CHECK("l2_prefetch_kernel");
-  return LADE_OK;
 }
 
 }  // extern "C"  (templated implementations below have C++ linkage)

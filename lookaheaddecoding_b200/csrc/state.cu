@@ -842,6 +842,6 @@ const char* lade_strerror(int code) {
 
 const char* lade_last_cuda_error(void) { return lade::g_last_error.c_str(); }
 
-int lade_version(void) { return 100; }
+int lade_version(void) { return 101; }
 
 }  // extern "C"

@@ -51,24 +51,9 @@ class LookaheadEngine:
 
     def __init__(self, model, window_size: int, level: int, guess_set_size: int,
                  pool_from_prompt: bool = False, max_total_len: int = 4096, attn_impl: int = 0,
-                 attn_splits: Optional[int] = None, use_cuda_graph: bool = True, debug: bool = False,
-                 dist_workers: int = 1, rank: int = 0, process_group=None, pipeline_host: bool = True,
-                 l2_prefetch: Optional[bool] = None, prefetch_mb: Optional[Sequence[float]] = None,
-                 prefetch_ctas: int = 32, prefetch_chunk: int = 32768):
+                 attn_splits: Optional[int] = None, use_cuda_graph: bool = True,
+                 dist_workers: int = 1, rank: int = 0, process_group=None, pipeline_host: bool = True):
         self.lib = _cabi.load()
-        # L2 weight prefetch on a side branch of the step graph (see _prefetch): MB of the NEXT projection's weights
-        # requested while [rmsnorm | rope+attention | rmsnorm | swiglu | final norm] run.  OFF unless asked for: the
-        # H100's 50 MB L2 holds little of one projection's weights, and no gain has been measured there.
-        import os as _os
-        if l2_prefetch is None:
-            l2_prefetch = _os.environ.get("LADE_L2_PREFETCH", "0") == "1"
-        self.l2_prefetch = bool(l2_prefetch)
-        env_mb = _os.environ.get("LADE_PREFETCH_MB")
-        if prefetch_mb is None and env_mb:
-            prefetch_mb = [float(x) for x in env_mb.split(",")]
-        self.prefetch_mb = tuple(prefetch_mb) if prefetch_mb is not None else (32.0, 110.0, 32.0, 36.0, 36.0)
-        self.prefetch_ctas, self.prefetch_chunk = int(prefetch_ctas), int(prefetch_chunk)
-        self._pf_stream = None
         self.pipeline_host = bool(pipeline_host)
         cfg = model.config
         p0 = next(model.parameters())
@@ -120,7 +105,6 @@ class LookaheadEngine:
                                 else getattr(cfg, "rope_theta", 10000.0))
         self.attn_impl = attn_impl
         self.use_cuda_graph = use_cuda_graph
-        self.debug = debug
         self.lm_cap = 1 + self.WCAP + self.G * self.GS
         # lookahead parallelism (lade_distributed): full replica per rank, window/guess slices per rank
         self.DW = int(dist_workers) if dist_workers and dist_workers > 1 else 1
@@ -172,7 +156,8 @@ class LookaheadEngine:
         self._pinned_ring = [torch.empty(_cabi.RES_INTS, dtype=torch.int32, pin_memory=True) for _ in range(2)]
         self._res_events = [torch.cuda.Event() for _ in range(2)]
         self.launches = 0   # kernels of THIS repo launched (graph replays counted by their content)
-        self._launches_per_graph = 0
+        # tests set a device float[>= 2 + G*(N-1) + W]: lade_sample_verify then records the uniforms it consumed
+        self.debug_uniforms: Optional[torch.Tensor] = None
         self.last_steps = 0
         self.last_records: List[StepRecord] = []
 
@@ -314,134 +299,102 @@ class LookaheadEngine:
 
     # ------------------------------------------------------------------------------------------
     def _launch_step(self, rows: int, stream: int, commit: bool = True, prefill: bool = False):
-        """All launches of one step on `stream` for `rows` materialised rows (rows <= rows_cap).
-        commit=False stops after the row-wise argmax (the sampling path decides on the host)."""
-        lib, L = self.lib, self.L
-        n = 0
-        skip = getattr(self, "_ablate", ())      # tools/step_ablation.py: leave kernels out to time the rest (results garbage)
-        # tests/rounding_attribution.py (checker, never set by the product): issue the projections call for call like the
-        # reference instead of fused / replace the attention launch, to attribute id differences to rounding order
-        unfused = getattr(self, "_unfused_gemms", False)
-        attn_hook = getattr(self, "_attn_hook", None)
+        """All launches of one step on `stream` (the current stream) for `rows` materialised rows (rows <= rows_cap).
+        Returns how many of this library's kernels were launched.  Each kernel family is a stage method below, so a
+        tool can replace one stage on its own engine instance."""
         # prefill (step 0) is plain causal and carries no rowmask; every later step has one and must fit it
         mw = 0 if prefill else self.mask_words
         if mw and rows > (mw - 1) * 32:
             raise LadeError(f"step of {rows} rows does not fit the {mw}-word row mask")
-        check(lib.lade_step_layout(self._ctx, stream, rows, _ptr(self.ids), _ptr(self.pos), _ptr(self.rowdesc),
-                                   _ptr(self.lm_rows), _ptr(self.meta), _ptr(self.rowmask) if mw else 0, mw),
-              "lade_step_layout"); n += 1
+        check(self.lib.lade_step_layout(self._ctx, stream, rows, _ptr(self.ids), _ptr(self.pos), _ptr(self.rowdesc),
+                                        _ptr(self.lm_rows), _ptr(self.meta), _ptr(self.rowmask) if mw else 0, mw),
+              "lade_step_layout"); n = 1
         h = self.h[:rows]
         torch.index_select(self.embed, 0, self.ids[:rows], out=h)
         xn, qkv, attn_out = self.xn[:rows], self.qkv[:rows], self.attn_out[:rows]
         o_buf, gu, act, d_buf = self.o_buf[:rows], self.gu[:rows], self.act[:rows], self.d_buf[:rows]
         qb = self.qb if rows == self.rows_cap else self.qb.view(-1)[: self.nh * rows * self.D].view(self.nh, rows, self.D)
         delta = None
-        kv_bound = self.attn_kv_bound
-        pf = self.prefetch_mb if (self.l2_prefetch and not prefill) else (0, 0, 0, 0, 0)
-        for l in range(L):
-            n += self._prefetch([(self.w_qkv[l], 0)], pf[0])                              # beside rmsnorm
-            if "norm" not in skip:
-                check(self.k_rmsnorm(stream, _ptr(h), _ptr(delta), _ptr(self.ln1[l]), _ptr(h) if delta is not None else 0,
-                                       _ptr(xn), rows, self.H, self.eps), "lade_rmsnorm"); n += 1
-            if "gemm" not in skip:
-                if unfused:      # the reference's three projections, call for call (modeling_llama.py:447-449)
-                    nq, nk = self.nh * self.D, self.nkv * self.D
-                    torch.mm(xn, self.w_qkv[l][:nq].t(), out=qkv[:, :nq])
-                    torch.mm(xn, self.w_qkv[l][nq:nq + nk].t(), out=qkv[:, nq:nq + nk])
-                    torch.mm(xn, self.w_qkv[l][nq + nk:].t(), out=qkv[:, nq + nk:])
-                else:
-                    torch.mm(xn, self.w_qkv[l].t(), out=qkv)
-            n += self._prefetch([(self.w_o[l], 0), (self.w_gu[l], 0)], pf[1])              # beside rope + attention
+        for l in range(self.L):
             kc, vc = self.kv[l, 0], self.kv[l, 1]
-            if "rope" not in skip:
-                check(self.k_rope_append(stream, _ptr(qkv), _ptr(self.cos), _ptr(self.sin), _ptr(self.pos), _ptr(self.meta),
-                                           _ptr(qb), _ptr(kc), _ptr(vc), rows, rows, self.nh, self.nkv, self.D,
-                                           self.kv_capacity, self.table_len), "lade_rope_append"); n += 1
-            if attn_hook is not None:
-                attn_hook(self, l, qb, kc, vc, attn_out, rows, prefill)
-            elif "attn" not in skip:
-                check(self.k_attn_fwd(stream, _ptr(qb), _ptr(kc), _ptr(vc), _ptr(attn_out), _ptr(self.rowmask) if mw else 0, mw,
-                                        _ptr(self.meta), _ptr(self.attn_scratch), rows, self.nh, self.nkv, self.D,
-                                        self.kv_capacity, kv_bound, self.attn_splits, self.attn_impl), "lade_attn_fwd"); n += 1
-            if "gemm" not in skip:
-                torch.mm(attn_out, self.w_o[l].t(), out=o_buf)
-            gu_done = max(0, int(pf[1] * 1e6) - self.w_o[l].numel() * 2) & ~15
-            n += self._prefetch([(self.w_gu[l], gu_done)], pf[2])                          # beside rmsnorm
-            if "norm" not in skip:
-                check(self.k_rmsnorm(stream, _ptr(h), _ptr(o_buf), _ptr(self.ln2[l]), _ptr(h), _ptr(xn), rows, self.H,
-                                       self.eps), "lade_rmsnorm"); n += 1
-            if "gemm" not in skip:
-                if unfused:      # gate_proj / up_proj separately (modeling_llama.py:378)
-                    torch.mm(xn, self.w_gu[l][: self.I].t(), out=gu[:, : self.I])
-                    torch.mm(xn, self.w_gu[l][self.I:].t(), out=gu[:, self.I:])
-                else:
-                    torch.mm(xn, self.w_gu[l].t(), out=gu)
-            n += self._prefetch([(self.w_down[l], 0)], pf[3])                              # beside swiglu
-            if "swiglu" not in skip:
-                check(self.k_swiglu(stream, _ptr(gu), _ptr(act), rows, self.I), "lade_swiglu"); n += 1
-            if "gemm" not in skip:
-                torch.mm(act, self.w_down[l].t(), out=d_buf)
+            n += self._norm(stream, h, delta, self.ln1[l], xn, rows)
+            n += self._proj(xn, self.w_qkv[l], qkv)
+            n += self._rope_append(stream, qkv, qb, kc, vc, rows)
+            n += self._attention(stream, l, qb, kc, vc, attn_out, rows, prefill)
+            n += self._proj(attn_out, self.w_o[l], o_buf)
+            n += self._norm(stream, h, o_buf, self.ln2[l], xn, rows)
+            n += self._proj(xn, self.w_gu[l], gu)
+            n += self._swiglu(stream, gu, act, rows)
+            n += self._proj(act, self.w_down[l], d_buf)
             delta = d_buf
-        n += self._prefetch([(self.lm_head, 0)], pf[4])                                    # beside the final norm
         check(self.k_rmsnorm_gather(stream, _ptr(h), _ptr(delta), _ptr(self.norm_w), _ptr(self.lm_rows),
                                       _ptr(self.xn_lm), self.lm_cap, self.H, self.eps), "lade_rmsnorm_gather"); n += 1
-        self._prefetch_join()
-        torch.mm(self.xn_lm, self.lm_head.t(), out=self.logits)
+        n += self._proj(self.xn_lm, self.lm_head, self.logits)
         check(self.k_argmax_rows(stream, _ptr(self.logits), self.lm_cap, self.V, self.V, _ptr(self.am)),
               "lade_argmax_rows"); n += 1
+        return n + self._commit(stream, commit)
+
+    def _norm(self, stream: int, h, delta, w, out, rows: int) -> int:
+        """out = rmsnorm(h + delta) * w; with a delta the residual sum is also written back to h."""
+        check(self.k_rmsnorm(stream, _ptr(h), _ptr(delta), _ptr(w), _ptr(h) if delta is not None else 0, _ptr(out),
+                             rows, self.H, self.eps), "lade_rmsnorm")
+        return 1
+
+    def _proj(self, x, w, out) -> int:
+        """out = x @ w^T for an nn.Linear weight `w` (every projection of the step, lm_head included)."""
+        torch.mm(x, w.t(), out=out)
+        return 0
+
+    def _rope_append(self, stream: int, qkv, qb, kc, vc, rows: int) -> int:
+        """RoPE on q and k; q to the head-major `qb`, k and v appended to the layer's cache."""
+        check(self.k_rope_append(stream, _ptr(qkv), _ptr(self.cos), _ptr(self.sin), _ptr(self.pos), _ptr(self.meta),
+                                 _ptr(qb), _ptr(kc), _ptr(vc), rows, rows, self.nh, self.nkv, self.D,
+                                 self.kv_capacity, self.table_len), "lade_rope_append")
+        return 1
+
+    def _attention(self, stream: int, l: int, qb, kc, vc, out, rows: int, prefill: bool) -> int:
+        """Lookahead attention of layer `l` over the cache and the step's rows (causal on prefill, row mask after)."""
+        mw = 0 if prefill else self.mask_words
+        check(self.k_attn_fwd(stream, _ptr(qb), _ptr(kc), _ptr(vc), _ptr(out), _ptr(self.rowmask) if mw else 0, mw,
+                              _ptr(self.meta), _ptr(self.attn_scratch), rows, self.nh, self.nkv, self.D,
+                              self.kv_capacity, self.attn_kv_bound, self.attn_splits, self.attn_impl), "lade_attn_fwd")
+        return 1
+
+    def _swiglu(self, stream: int, gu, out, rows: int) -> int:
+        """out = silu(gate) * up on the fused gate/up projection."""
+        check(self.k_swiglu(stream, _ptr(gu), _ptr(out), rows, self.I), "lade_swiglu")
+        return 1
+
+    def _commit(self, stream: int, commit) -> int:
+        """State update at the end of the step, by `commit`:
+        False: none (the sampling path decides on the host);
+        "sample": verification + residual draw on device (Philox), then the decision's commit and KV compaction;
+        True on one GPU: fused verify + accept + update, then KV compaction;
+        True under LP: the local verify, then the exchange and the replicated commit when NCCL runs in the library
+        (otherwise generate() calls _lp_commit outside the step)."""
+        lib = self.lib
         if not commit:
-            return n
-        if commit == "sample":      # verification + residual draw on device (Philox), then the state update
+            return 0
+        if commit == "sample":
             check(self.k_sample_verify(self._ctx, stream, _ptr(self.logits), self.V, self.V, _ptr(self.am), _ptr(self.meta),
-                                         float(self.sample_temperature), int(self.sample_top_k), float(self.sample_top_p),
-                                         _ptr(self.rng_state), _ptr(self.dec_dev),
-                                         _ptr(getattr(self, "debug_uniforms", None))),
+                                       float(self.sample_temperature), int(self.sample_top_k), float(self.sample_top_p),
+                                       _ptr(self.rng_state), _ptr(self.dec_dev), _ptr(self.debug_uniforms)),
                   "lade_sample_verify")
             check(lib.lade_commit_decision(self._ctx, stream, _ptr(self.dec_dev), _ptr(self.meta), _ptr(self.res)),
                   "lade_commit_decision")
-            check(lib.lade_kv_compact(stream, _ptr(self.res), _ptr(self.kv[0, 0]), _ptr(self.kv[0, 1]),
-                                      self.kv.stride(0), self.L, self.nkv, self.kv_capacity, self.D, max(self.GS - 1, 1)),
-                  "lade_kv_compact")
-            return n + 3
-        if self.DW == 1:
-            n += self._launch_commit(stream)
-        else:   # LP: local verify, then the exchange + replicated commit (in the same graph when NCCL is in-library)
+            n = 2
+        elif self.DW == 1:
+            check(lib.lade_accept_update(self._ctx, stream, _ptr(self.am), _ptr(self.meta), _ptr(self.res)),
+                  "lade_accept_update")
+            n = 1
+        else:
             check(lib.lade_lp_verify(self._ctx, stream, _ptr(self.am), _ptr(self.meta), _ptr(self.lp_send)),
-                  "lade_lp_verify"); n += 1
-            if self._nccl_comm:
-                n += self._launch_commit(stream)
-        return n
-
-    def _prefetch(self, pieces, budget_mb: float) -> int:
-        """Fork: queue an L2 prefetch of up to `budget_mb` MB of `pieces` ([(tensor, byte offset)] in consumption
-        order) on the side stream, ordered after everything queued on the current stream so far, so that it runs
-        BESIDE the kernels queued next (norm / RoPE / attention / SwiGLU: HBM idle).  Returns #kernels launched."""
-        if not self.l2_prefetch or budget_mb <= 0:
-            return 0
-        cur = torch.cuda.current_stream(self.dev)
-        if self._pf_stream is None:
-            self._pf_stream = torch.cuda.Stream(device=self.dev)
-        self._pf_stream.wait_stream(cur)
-        left = int(budget_mb * 1e6)
-        n = 0
-        for t, off in pieces:
-            nbytes = (min(left, t.numel() * t.element_size() - off)) & ~15
-            if nbytes <= 0:
-                continue
-            check(self.lib.lade_l2_prefetch(self._pf_stream.cuda_stream, t.data_ptr() + off, nbytes, self.prefetch_ctas,
-                                            self.prefetch_chunk), "lade_l2_prefetch")
-            n += 1
-            left -= nbytes
-            if left <= 0:
-                break
-        self._pf_dirty = True
-        return n
-
-    def _prefetch_join(self) -> None:
-        """Join the side branch back (a captured graph must end on its origin stream)."""
-        if self._pf_stream is not None and getattr(self, "_pf_dirty", False):
-            torch.cuda.current_stream(self.dev).wait_stream(self._pf_stream)
-            self._pf_dirty = False
+                  "lade_lp_verify")
+            return 1 + (self._lp_commit(stream) if self._nccl_comm else 0)
+        check(lib.lade_kv_compact(stream, _ptr(self.res), _ptr(self.kv[0, 0]), _ptr(self.kv[0, 1]),
+                                  self.kv.stride(0), self.L, self.nkv, self.kv_capacity, self.D, max(self.GS - 1, 1)),
+              "lade_kv_compact")
+        return n + 1
 
     def _lp_comm_create(self) -> None:
         """In-library NCCL communicator for the per-step record exchange (lade_lp_exchange): rank 0 draws the unique
@@ -468,24 +421,16 @@ class LookaheadEngine:
     def lp_in_library(self) -> bool:
         return bool(self._nccl_comm)
 
-    def _launch_commit(self, stream: int) -> int:
-        """State update of the step.  Single GPU: fused verify+accept+update, then KV compaction.
-        LP: one all-gather of the fixed-size per-rank records over NCCL, then the replicated commit."""
-        lib = self.lib
-        if self.DW == 1:
-            check(lib.lade_accept_update(self._ctx, stream, _ptr(self.am), _ptr(self.meta), _ptr(self.res)),
-                  "lade_accept_update")
-            check(lib.lade_kv_compact(stream, _ptr(self.res), _ptr(self.kv[0, 0]), _ptr(self.kv[0, 1]),
-                                      self.kv.stride(0), self.L, self.nkv, self.kv_capacity, self.D, max(self.GS - 1, 1)),
-                  "lade_kv_compact")
-            return 2
+    def _lp_commit(self, stream: int) -> int:
+        """LP: one all-gather of the fixed-size per-rank records, then the replicated commit."""
         if self._nccl_comm:      # ncclAllGather on the compute stream, inside the library (graph-capturable)
-            check(lib.lade_lp_exchange(self._ctx, stream, self._nccl_comm, _ptr(self.lp_send), _ptr(self.lp_recv)),
+            check(self.lib.lade_lp_exchange(self._ctx, stream, self._nccl_comm, _ptr(self.lp_send), _ptr(self.lp_recv)),
                   "lade_lp_exchange")
         else:
             import torch.distributed as dist
             dist.all_gather_into_tensor(self.lp_recv, self.lp_send, group=self.pg)
-        check(lib.lade_lp_commit(self._ctx, stream, _ptr(self.lp_recv), _ptr(self.meta), _ptr(self.res)), "lade_lp_commit")
+        check(self.lib.lade_lp_commit(self._ctx, stream, _ptr(self.lp_recv), _ptr(self.meta), _ptr(self.res)),
+              "lade_lp_commit")
         return 1
 
     @staticmethod
@@ -526,7 +471,6 @@ class LookaheadEngine:
                 n = self._launch_step(rows, torch.cuda.current_stream(self.dev).cuda_stream, commit=commit)
         torch.cuda.current_stream(self.dev).wait_stream(side)
         self._graph[key] = (g, n)
-        self._launches_per_graph = n
         self._graph_n = n
         return g
 
@@ -625,7 +569,7 @@ class LookaheadEngine:
             nonlocal queued
             self.run_forward_step(queued, P, commit=commit)
             if self.DW > 1 and not self._nccl_comm:       # torch all-gather fallback: outside the graph
-                self.launches += self._launch_commit(stream)
+                self.launches += self._lp_commit(stream)
             slot = queued & 1
             self._enqueue_result_copy(slot)
             inflight.append(slot)

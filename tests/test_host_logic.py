@@ -234,4 +234,3 @@ def test_nccl_entry_points_degrade_without_a_communicator():
     assert lib.lade_nccl_comm_destroy(None) == _cabi.LADE_EINVAL
     assert lib.lade_lp_exchange(None, None, None, None, None) == _cabi.LADE_EINVAL
     assert lib.lade_sample_verify(None, None, None, 0, 0, None, None, C.c_float(1.0), 0, C.c_float(1.0), None, None, None) == _cabi.LADE_EINVAL
-    assert lib.lade_l2_prefetch(None, None, 0, 1, 16) == _cabi.LADE_EINVAL

@@ -2,7 +2,8 @@
 """Where does the steady decode step go, IN the graph (warm caches, real launch gaps)?  ncu serialises and flushes,
 so its per-kernel times overstate the small kernels.  Here the captured step graph is rebuilt with one kernel family
 left out at a time (results are garbage, timing is not) and replayed back to back; the difference to the full step is
-what that family costs in situ, launch gaps included."""
+what that family costs in situ, launch gaps included.  A family is left out by replacing the engine's stage method with
+a no-op; `gemm` is every projection, the lm_head GEMM included."""
 import json
 import os
 import random
@@ -13,6 +14,8 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
 from lookaheaddecoding_b200 import LookaheadEngine  # noqa: E402
+
+STAGES = {"norm": "_norm", "gemm": "_proj", "rope": "_rope_append", "attn": "_attention", "swiglu": "_swiglu"}
 
 
 @torch.no_grad()
@@ -26,15 +29,20 @@ def main():
     prompt = torch.randint(3, shape["vocab"], (P,)).tolist()
     eng.generate(prompt, 130, rng=random.Random(0))       # kv ~ 1150 afterwards: mid-run context
 
-    def graph_ms(ablate, reps=60):
-        eng._ablate = set(ablate)
+    def ablate(families):
+        for name in STAGES.values():                       # instance attributes shadow the class's stage methods
+            eng.__dict__.pop(name, None)
+        for f in families:
+            setattr(eng, STAGES[f], lambda *args: 0)
+
+    def graph_ms(families, reps=60):
         eng._graph = None
         eng.begin(prompt, P + new, (), eng.draw_window(prompt, random.Random(0), None))
-        eng._ablate = set()
+        ablate(())
         for s in range(N - 2):                             # real prefill + window fill so that kv_len / phase are steady
             eng.run_forward_step(s, P)
             eng._read_result()
-        eng._ablate = set(ablate)
+        ablate(families)
         g = eng._steady_graph(True)
         for _ in range(5):
             g.replay()
@@ -45,7 +53,7 @@ def main():
             g.replay()
         e1.record()
         torch.cuda.synchronize()
-        eng._ablate = set()
+        ablate(())
         return e0.elapsed_time(e1) / reps
 
     full = graph_ms(())
