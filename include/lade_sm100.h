@@ -172,12 +172,16 @@ int lade_attn_fwd(void* stream, const void* q, const void* k_cache, const void* 
                   int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, int32_t kv_capacity,
                   int32_t kv_bound /* host upper bound of kv_len + q_len */, int32_t n_splits,
                   int32_t impl /* 0 = default (= 2), 1 = mma.sync path, 2 = wgmma/TMA path, 3 = its reference-order variant */);
-/* Bytes of zero-initialised scratch `lade_attn_fwd` needs for a shape (impl 1 keeps split partials there; the
- * wgmma path merges inside the cluster and only needs the buffer to exist).  No reference counterpart. */
+/* Bytes of zero-initialised scratch `lade_attn_fwd` needs for a shape.  Every impl merges its KV splits through it:
+ * [16384 int32 ticket counters, one per (head, q tile), zero at rest][(m, l) fp32 per split row][fp32 O per split row],
+ * split-major, rows padded to 128.  Each split writes its partial rows and takes a ticket; the CTA that draws the last
+ * one combines the splits and puts the counter back to 0, so the buffer needs no clearing between launches.  impl 3
+ * also exchanges its row maxima and row sums through the (m, l) table.  Launches that share a scratch buffer must be
+ * stream-ordered.  No reference counterpart. */
 int64_t lade_attn_scratch_bytes(int32_t q_pad, int32_t n_heads, int32_t head_dim, int32_t n_splits);
 /* Profiling aid: when set (device buffer of 16 int64 per CTA, or NULL to disable) the wgmma kernel records
- * clock64() at its phase boundaries (start, first K tile landed, first S ready, O final, partials written,
- * siblings arrived, merged, end). */
+ * %globaltimer (ns) at its phase boundaries in slots 0-7 (start, first K tile landed, first S ready, O final, partials
+ * written, ticket drawn, -, end) and the SM it ran on in slot 15. */
 int lade_debug_attn_timing(void* dev_buffer);
 
 /* Measurement aid: force the programmatic-dependent-launch attribute of lade_attn_fwd on (1) / off (0), or back to the

@@ -1,5 +1,5 @@
 // Lookahead attention, Hopper-native path (impl=2): TMA-staged K/V tiles, wgmma with register accumulators, the
-// lookahead mask evaluated in registers, split-KV across a thread-block cluster with an in-kernel merge.
+// lookahead mask evaluated in registers, split-KV with an in-kernel merge through L2.
 //
 // Per CTA: one (head, 128-row query tile, KV split).  Warp roles (288 threads):
 //   warps 0..7   two consumer warpgroups, 64 query rows each:
@@ -9,7 +9,10 @@
 //                  O += P V     (wgmma m64n128k16, P from registers, V from shared memory, MN-major)
 //   warp 8       TMA producer: Q tile + a 3-deep ring of K/V tiles (128 kv rows x 128 d, SWIZZLE_128B); it also zeroes
 //                the stale cache rows past kv_len + q_len of the last V tile (0 * NaN must not reach the MMA)
-// Split merge: fp32 partial rows pushed from registers into the owner CTA's shared memory (st.shared::cluster).
+// Split merge: every split writes its fp32 partial rows to the scratch and takes a ticket on a per-(head, q tile)
+// counter; the last CTA to arrive combines them in a fixed order.  The splits need not be co-resident, so impl 2 is a
+// plain grid: a cluster of 4 one-SM CTAs must fit inside one GPC, and on an H100 SXM with 132 SMs only 30 such clusters
+// fit at once -- the 32 heads of the decode step then ran in two rounds.
 //
 // Numerics follow attn_mma.cu / the reference (lade/models/modeling_llama.py:520-541); the mask is the
 // same register predicate (common.cuh row_sees == modeling_llama.py:115-207).
@@ -43,16 +46,25 @@ constexpr int TC_HALF_BYTES = TC_TILE_BYTES / 2;
 constexpr int TC_SMEM_TILES = TC_TILE_BYTES * (1 + 2 * TC_STAGES);
 constexpr int TC_SMEM_BYTES = TC_SMEM_TILES + 256 + 1024;   // tiles + mbarriers + slack to align the base to 1024 B
 constexpr float TC_LOG2E = 1.4426950408889634f;
-// DSMEM merge: slots of [per][TC_SO_STRIDE] floats alias the owner's dead K/V stages, the (m, l) table its dead Q tile
-// (a cluster barrier separates compute from the pushes); (n - 1) * ceil(128 / n) * 528 B <= 59,136 for n <= 8.
-constexpr int TC_SO_STRIDE = 132;                       // floats per staged O row (528 B)
-constexpr int TC_SO_OFFSET = TC_TILE_BYTES;
-constexpr int TC_SML_OFFSET = 0;
+// Split merge: [counters: TC_MAX_COUNTERS ints, zero at rest][part_ml: (m, l) per split row][part_o: fp32 O per split
+// row] at the start of the caller's scratch (lade_attn_scratch_bytes), the layout of the mma.sync kernel's merge.
+constexpr int TC_MAX_COUNTERS = 16384;
 
-// Optional per-CTA phase timestamps (clock64) for profiling the kernel's own timeline: 16 slots per CTA, 0-7 used.
+// Optional per-CTA phase timestamps for profiling the kernel's own timeline: 16 slots per CTA, 0-7 hold %globaltimer
+// (ns, one clock for the whole GPU, so CTAs on different SMs compare), 15 the SM the CTA ran on.
 __device__ long long* g_attn_timing = nullptr;
-#define TC_STAMP(slot, tid) do { if (tbuf && threadIdx.x == (tid)) tbuf[slot] = clock64(); } while (0)
-enum { TS_START = 0, TS_KFULL0 = 1, TS_SFULL0 = 2, TS_OFINAL = 3, TS_STAGED = 4, TS_CLUSTER = 5, TS_MERGED = 6, TS_END = 7 };
+__device__ __forceinline__ long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return (long long)t;
+}
+__device__ __forceinline__ int sm_id() {
+  int s;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+  return s;
+}
+#define TC_STAMP(slot, tid) do { if (tbuf && threadIdx.x == (tid)) tbuf[slot] = global_ns(); } while (0)
+enum { TS_START = 0, TS_KFULL0 = 1, TS_SFULL0 = 2, TS_OFINAL = 3, TS_STAGED = 4, TS_TICKET = 5, TS_END = 7, TS_SMID = 15 };
 
 // The model-dtype pair packed by Elem<ET>::pack2, back in fp32 (the rounded probabilities the row sum adds up).
 template <typename ET> __device__ __forceinline__ float2 unpack2(uint32_t u);
@@ -109,14 +121,15 @@ __device__ __forceinline__ bool vis(const uint32_t (&mb)[2][4], int rr, int i, i
 }
 
 // ---- kernel ---------------------------------------------------------------------------------------------
-// grid (n_splits, heads, q tiles); the n_splits CTAs of one (head, q tile) form a thread-block cluster and merge their
-// split-KV partials through distributed shared memory.
+// grid (n_splits, heads, q tiles); the n_splits CTAs of one (head, q tile) merge their split-KV partials through the
+// scratch (impl 3 launches them as a thread-block cluster for its two mid-kernel exchanges).
 template <typename ET, bool REF>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, ET* __restrict__ out,
                    const uint32_t* __restrict__ rowmask, int mask_words, const int* __restrict__ meta, int q_pad,
-                   int n_heads, int n_kv_heads, int n_splits, float inv_sqrt_d, float2* __restrict__ row_ml) {
+                   int n_heads, int n_kv_heads, int n_splits, float inv_sqrt_d, int* __restrict__ counters,
+                   float2* __restrict__ part_ml, float* __restrict__ part_o) {
   extern __shared__ unsigned char smem_raw[];
   const uint32_t raw_a = smem_u32(smem_raw);
   const uint32_t sQ_a = (raw_a + 1023u) & ~1023u;                  // SWIZZLE_128B tiles need 1024-byte alignment
@@ -141,13 +154,16 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   if (REF && t_base + (t_rem ? 1 : 0) > TC_STAGES) __trap();     // the caller's kv_bound was not a bound (host checks it)
   const int hk = h / (n_heads / n_kv_heads);
   const int HD = n_heads * TC_D;
-  const long long hm = (long long)h * gridDim.z + mt;
+  // split-major scratch tables: row r of this tile is row prow0 + r of split s's slab
+  const long long slab = (long long)n_heads * gridDim.z * TC_BM;
+  const long long prow0 = ((long long)h * gridDim.z + mt) * TC_BM;
   // a warpgroup whose 64 rows are all padding has nothing to compute
   const int n_wg = (mt * TC_BM + 64 < q_pad) ? 2 : 1;
   // the last tile of the launch may run past kv_len + q_len: its stale V rows are zeroed before P.V reads them
   const bool zero_last = active && (tile_lo + my_tiles) * TC_BN > T;
   long long* tbuf = g_attn_timing ? g_attn_timing + 16ll * ((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
   TC_STAMP(TS_START, 0);
+  if (tbuf && threadIdx.x == 0) tbuf[TS_SMID] = sm_id();
   // programmatic dependent launch, producer side: a dependent grid may be scheduled as soon as SMs free up; it orders
   // itself with griddepcontrol.wait before it touches anything this grid writes
   griddep_launch_dependents();
@@ -194,6 +210,10 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int j = n_old; j < n_pre; ++j) issue_tile(j);
   }
   __syncthreads();
+  // Every thread that writes the scratch (split partials, (m, l) rows, the ticket counters) is ordered after the
+  // predecessor grid here: under programmatic dependent launch that grid may be the previous attention launch, which
+  // uses the same scratch.  In an active CTA the producer thread has already waited, so this returns at once.
+  griddep_wait();
 
   // a consumer thread's share of its split's result: two rows (g and g + 8 of its warp's 16) x 32 of the 128 columns,
   // the unnormalised O (impl 2) or the normalised partial O (impl 3); kept in registers for the split merge
@@ -330,7 +350,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 1));
           mx[rr] = fmaxf(mx[rr], __shfl_xor_sync(0xffffffffu, mx[rr], 2));
           const float m_split = mx[rr] == -INFINITY ? -INFINITY : round_to<ET>(round_to<ET>(mx[rr]) * inv_sqrt_d);
-          if (t == 0) row_ml[(hm * n_splits + split) * TC_BM + rl[rr]].x = m_split;
+          if (t == 0) part_ml[split * slab + prow0 + rl[rr]].x = m_split;
         }
       }
       cluster_arrive(); cluster_wait();
@@ -340,7 +360,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         for (int rr = 0; rr < 2; ++rr) {
           float m_all = -INFINITY;
           for (int sp = 0; sp < n_active; ++sp)
-            m_all = fmaxf(m_all, ld_global_f2(row_ml + (hm * n_splits + sp) * TC_BM + rl[rr]).x);
+            m_all = fmaxf(m_all, ld_global_f2(part_ml + sp * slab + prow0 + rl[rr]).x);
           m_ref[rr] = (m_all == -INFINITY) ? 0.f : m_all;   // x - max is exact in fp32 (both are model-dtype values)
         }
       }
@@ -375,7 +395,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         for (int rr = 0; rr < 2; ++rr) {
           l_part[rr] += __shfl_xor_sync(0xffffffffu, l_part[rr], 1);
           l_part[rr] += __shfl_xor_sync(0xffffffffu, l_part[rr], 2);
-          if (t == 0) row_ml[(hm * n_splits + split) * TC_BM + rl[rr]].y = l_part[rr];
+          if (t == 0) part_ml[split * slab + prow0 + rl[rr]].y = l_part[rr];
         }
       }
       cluster_arrive(); cluster_wait();
@@ -383,7 +403,7 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       if (work) {
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr)
-          for (int sp = 0; sp < n_active; ++sp) l_all[rr] += ld_global_f2(row_ml + (hm * n_splits + sp) * TC_BM + rl[rr]).y;
+          for (int sp = 0; sp < n_active; ++sp) l_all[rr] += ld_global_f2(part_ml + sp * slab + prow0 + rl[rr]).y;
       }
       // ---- pass C: p = model_dtype(e / sum) -> P.V, tile by tile
       for (int j = 0; work && j < my_tiles; ++j) {
@@ -413,83 +433,119 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       }
     }
   }
-  TC_STAMP(TS_STAGED, 0);
   if (n_splits == 1) { TC_STAMP(TS_END, 0); return; }
+  if (!active) return;                                // a split without tiles takes no part in the merge
 
-  // ---- split merge across the cluster ----
-  // Row r of the tile is owned by CTA r / per (per = ceil(rows / n_active)); only the tile's real rows (row < q_pad)
-  // travel.  Threads of foreign rows store their registers straight into the owner CTA's shared memory
-  // (st.shared::cluster, fire and forget); barrier 1 = every CTA is done with its stages, barrier 2 = the pushes have
-  // landed; the owner threads then combine their own registers with the slots from LOCAL shared memory:
-  //   impl 2:  w_s = 2^(m_s - m),  out = sum_s w_s O_s / sum_s w_s l_s        impl 3:  out = sum_s O_s
+  // ---- split merge through L2, by the CTA that arrives last ----
+  // Every split stores its partial rows (fp32 O; impl 2 also (m, l)) in the scratch, fences, and takes a ticket on the
+  // (head, q tile) counter; the CTA that draws the last ticket combines all of them and puts the counter back to 0.
+  // Row r of the tile is combined in a fixed order: its owning split r / per (per = ceil(rows / n_active)) first, then
+  // the others in ascending split order, every step rounded as written (no contraction can move a bit):
+  //   impl 2:  w_s = 2^(m_s - m),  out = (sum_s w_s O_s) * (1 / sum_s w_s l_s)        impl 3:  out = sum_s O_s
+  // A single active split is its own last CTA and merges from registers.
   const int rows_valid = min(TC_BM, q_pad - mt * TC_BM);
   const int per = (rows_valid + n_active - 1) / n_active;
-  cluster_arrive();
-  cluster_wait();
-  TC_STAMP(TS_CLUSTER, 0);
-  int dest[2] = {-1, -1}, r_in[2] = {0, 0};
-  if (work) {
+  int* const counter = counters + h * gridDim.z + mt;
+  if (n_active > 1) {
+    __shared__ int s_last;
+    if (work) {
 #pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      dest[rr] = rl[rr] < rows_valid ? rl[rr] / per : -2;
-      r_in[rr] = rl[rr] - dest[rr] * per;
-      if (dest[rr] >= 0 && dest[rr] != split) {
-        const int slot = split < dest[rr] ? split : split - 1;
-        const uint32_t o_a = dsmem_addr(sQ_a + TC_SO_OFFSET + (uint32_t)(((slot * per + r_in[rr]) * TC_SO_STRIDE + 2 * t) * 4), dest[rr]);
+      for (int rr = 0; rr < 2; ++rr) {
+        if (rl[rr] >= rows_valid) continue;
+        float2* po = reinterpret_cast<float2*>(part_o + (split * slab + prow0 + rl[rr]) * TC_D + 2 * t);
 #pragma unroll
-        for (int i = 0; i < 16; ++i) st_dsmem_f2(o_a + i * 32, o[4 * i + 2 * rr], o[4 * i + 2 * rr + 1]);
-        if (!REF && t == 0)
-          st_dsmem_f2(dsmem_addr(sQ_a + TC_SML_OFFSET + (uint32_t)((slot * per + r_in[rr]) * 8), dest[rr]), m_row[rr], l_row[rr]);
+        for (int i = 0; i < 16; ++i) po[4 * i] = make_float2(o[4 * i + 2 * rr], o[4 * i + 2 * rr + 1]);
+        if (!REF && t == 0) part_ml[split * slab + prow0 + rl[rr]] = make_float2(m_row[rr], l_row[rr]);
       }
     }
+    TC_STAMP(TS_STAGED, 0);
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = atomicAdd(counter, 1) == n_active - 1;
+    __syncthreads();
+    TC_STAMP(TS_TICKET, 0);
+    if (!s_last) return;
+    __threadfence();
+    if (threadIdx.x == 0) *counter = 0;             // every split has drawn its ticket: ready for the next launch
   }
-  cluster_arrive();
-  cluster_wait();
-  TC_STAMP(TS_MERGED, 0);
-  if (work) {
-    const float2* sml = reinterpret_cast<const float2*>(smem + TC_SML_OFFSET);
-    const float* so = reinterpret_cast<const float*>(smem + TC_SO_OFFSET);
+  if (work && n_active == 1) {                        // the partial is the result: it never left the registers
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
-      if (dest[rr] != split) continue;
-      float inv = 1.f;
+      if (rl[rr] >= rows_valid) continue;
+      float wgt = 1.f, inv = 1.f;
       if (!REF) {
-        float mmax = m_row[rr];
-        for (int k = 0; k < n_active - 1; ++k) mmax = fmaxf(mmax, sml[k * per + r_in[rr]].x);
-        float wgt = (m_row[rr] == -INFINITY) ? 0.f : exp2f((m_row[rr] - mmax) * TC_LOG2E);
-        float lsum = l_row[rr] * wgt;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) { o[4 * i + 2 * rr] *= wgt; o[4 * i + 2 * rr + 1] *= wgt; }
-        for (int k = 0; k < n_active - 1; ++k) {
-          const float2 ml = sml[k * per + r_in[rr]];
-          wgt = (ml.x == -INFINITY) ? 0.f : exp2f((ml.x - mmax) * TC_LOG2E);
-          lsum += ml.y * wgt;
-          const float* src = so + (k * per + r_in[rr]) * TC_SO_STRIDE + 2 * t;
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float2 x = *reinterpret_cast<const float2*>(src + 8 * i);
-            o[4 * i + 2 * rr] += x.x * wgt;
-            o[4 * i + 2 * rr + 1] += x.y * wgt;
-          }
-        }
+        wgt = (m_row[rr] == -INFINITY) ? 0.f : exp2f((m_row[rr] - m_row[rr]) * TC_LOG2E);
+        const float lsum = __fmul_rn(l_row[rr], wgt);
         inv = lsum > 0.f ? 1.f / lsum : 0.f;
-      } else {
-        for (int k = 0; k < n_active - 1; ++k) {
-          const float* src = so + (k * per + r_in[rr]) * TC_SO_STRIDE + 2 * t;
+      }
+      uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)(mt * TC_BM + rl[rr]) * HD + h * TC_D + 2 * t);
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+        dst[4 * i] = Elem<ET>::pack2(__fmul_rn(__fmul_rn(o[4 * i + 2 * rr], wgt), inv),
+                                     __fmul_rn(__fmul_rn(o[4 * i + 2 * rr + 1], wgt), inv));
+    }
+  } else if (work) {
+    // Both rows of the thread advance together and every split's rows are loaded before they are used, so the merge
+    // costs about n_active + 1 L2 round trips.  The CTA's own partial is read back from L2 like the others.
+    bool valid[2];
+    int own[2];
+    const float2* pml[2];
+    const float2* po[2];
+    float mmax[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      valid[rr] = rl[rr] < rows_valid;
+      own[rr] = rl[rr] / per;
+      pml[rr] = part_ml + prow0 + rl[rr];
+      po[rr] = reinterpret_cast<const float2*>(part_o + (prow0 + rl[rr]) * TC_D + 2 * t);
+      mmax[rr] = -INFINITY;                          // max over the splits: exact, so its order does not matter
+      if (!REF && valid[rr]) {
+        float mx[8];
+#pragma unroll
+        for (int s = 0; s < 8; ++s) mx[s] = s < n_active ? __ldcg(pml[rr] + s * slab).x : -INFINITY;
+#pragma unroll
+        for (int s = 0; s < 8; ++s) mmax[rr] = fmaxf(mmax[rr], mx[s]);
+      }
+    }
+    float acc[2][32], lsum[2] = {0.f, 0.f};
+    for (int k = 0; k < n_active; ++k) {
+      float2 x[2][16], ml[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {               // the owning split first, then the others in ascending order
+        const int s = k == 0 ? own[rr] : (k - 1 < own[rr] ? k - 1 : k);
+        if (!valid[rr]) continue;
+        if (!REF) ml[rr] = __ldcg(pml[rr] + s * slab);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) x[rr][i] = __ldcg(po[rr] + s * slab * (TC_D / 2) + 4 * i);
+      }
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        if (!valid[rr]) continue;
+        if (!REF) {
+          const float wgt = (ml[rr].x == -INFINITY) ? 0.f : exp2f((ml[rr].x - mmax[rr]) * TC_LOG2E);
+          lsum[rr] = k == 0 ? __fmul_rn(ml[rr].y, wgt) : __fmaf_rn(ml[rr].y, wgt, lsum[rr]);
 #pragma unroll
           for (int i = 0; i < 16; ++i) {
-            const float2 x = *reinterpret_cast<const float2*>(src + 8 * i);
-            o[4 * i + 2 * rr] += x.x;
-            o[4 * i + 2 * rr + 1] += x.y;
+            acc[rr][2 * i] = k == 0 ? __fmul_rn(x[rr][i].x, wgt) : __fmaf_rn(x[rr][i].x, wgt, acc[rr][2 * i]);
+            acc[rr][2 * i + 1] = k == 0 ? __fmul_rn(x[rr][i].y, wgt) : __fmaf_rn(x[rr][i].y, wgt, acc[rr][2 * i + 1]);
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            acc[rr][2 * i] = k == 0 ? x[rr][i].x : __fadd_rn(acc[rr][2 * i], x[rr][i].x);
+            acc[rr][2 * i + 1] = k == 0 ? x[rr][i].y : __fadd_rn(acc[rr][2 * i + 1], x[rr][i].y);
           }
         }
       }
-      const int row = mt * TC_BM + rl[rr];
-      if (row < q_pad) {
-        uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)row * HD + h * TC_D + 2 * t);
+    }
 #pragma unroll
-        for (int i = 0; i < 16; ++i) dst[4 * i] = Elem<ET>::pack2(o[4 * i + 2 * rr] * inv, o[4 * i + 2 * rr + 1] * inv);
-      }
+    for (int rr = 0; rr < 2; ++rr) {
+      if (!valid[rr]) continue;
+      const float inv = REF ? 1.f : (lsum[rr] > 0.f ? 1.f / lsum[rr] : 0.f);
+      uint32_t* dst = reinterpret_cast<uint32_t*>(out + (long long)(mt * TC_BM + rl[rr]) * HD + h * TC_D + 2 * t);
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+        dst[4 * i] = Elem<ET>::pack2(__fmul_rn(acc[rr][2 * i], inv), __fmul_rn(acc[rr][2 * i + 1], inv));
     }
   }
   TC_STAMP(TS_END, 0);
@@ -565,12 +621,15 @@ static bool pdl_enabled() {
   return v != 0;
 }
 
-// One launch of attn_fwd_tc_kernel<ET, REF>: grid (n_splits, heads, q tiles), the splits of a (head, q tile) a cluster.
+// One launch of attn_fwd_tc_kernel<ET, REF>: grid (n_splits, heads, q tiles).  The reference-order variant meets its
+// sibling splits twice in the middle of the kernel, so the splits of a (head, q tile) form a cluster (co-resident);
+// impl 2 needs no co-residency and is launched as a plain grid.
 template <typename ET, bool REF>
 static int launch_tc(cudaStream_t stream, const void* q, const void* k_cache, const void* v_cache, void* out,
                      const uint32_t* rowmask, int mask_words, const int32_t* meta, void* scratch, int q_pad, int n_heads,
                      int n_kv_heads, int head_dim, int kv_capacity, int n_splits) {
   const int q_tiles = (q_pad + TC_BM - 1) / TC_BM;
+  if ((long long)n_heads * q_tiles > TC_MAX_COUNTERS) return LADE_EUNSUPPORTED;
   if ((reinterpret_cast<uintptr_t>(q) & 15) || (reinterpret_cast<uintptr_t>(k_cache) & 15) ||
       (reinterpret_cast<uintptr_t>(v_cache) & 15))
     return LADE_EINVAL;
@@ -592,23 +651,28 @@ static int launch_tc(cudaStream_t stream, const void* q, const void* k_cache, co
   cfg.dynamicSmemBytes = TC_SMEM_BYTES;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;   // the splits of one (head, q tile) form a cluster
-  attr[0].val.clusterDim.x = n_splits;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
+  int n_attr = 0;
   // programmatic dependent launch: the grid may start while its stream predecessor (lade_rope_append, which signals
   // griddepcontrol.launch_dependents at entry) is still running; the kernel orders itself with griddepcontrol.wait
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  if (pdl_enabled()) {
+    attr[n_attr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n_attr++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (REF) {
+    attr[n_attr].id = cudaLaunchAttributeClusterDimension;
+    attr[n_attr].val.clusterDim.x = n_splits;
+    attr[n_attr].val.clusterDim.y = 1;
+    attr[n_attr++].val.clusterDim.z = 1;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
+  cfg.numAttrs = n_attr;
   const float inv_sqrt_d = 1.0f / sqrtf((float)head_dim);
-  // scratch (lade_attn_scratch_bytes): [64 KB reserved][n_splits * n_heads * rows_pad * D fp32][(m, l) per row]; the
-  // reference-order variant exchanges its row maxima and sums through the (m, l) table
-  float* part_o = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) + 65536);
-  float2* row_ml = reinterpret_cast<float2*>(part_o + (size_t)n_splits * n_heads * q_tiles * TC_BM * TC_D);
+  // scratch (lade_attn_scratch_bytes): [counters][part_ml][part_o] with n_splits * n_heads * q_tiles * 128 rows per table
+  int* counters = reinterpret_cast<int*>(scratch);
+  float2* part_ml = reinterpret_cast<float2*>(counters + TC_MAX_COUNTERS);
+  float* part_o = reinterpret_cast<float*>(part_ml + (size_t)n_splits * n_heads * q_tiles * TC_BM);
   cudaError_t e = cudaLaunchKernelEx(&cfg, attn_fwd_tc_kernel<ET, REF>, tmQ, tmK, tmV, (ET*)out, rowmask, mask_words, meta,
-                                     q_pad, n_heads, n_kv_heads, n_splits, inv_sqrt_d, row_ml);
+                                     q_pad, n_heads, n_kv_heads, n_splits, inv_sqrt_d, counters, part_ml, part_o);
   if (e != cudaSuccess) { set_cuda_error(e, "cudaLaunchKernelEx(attn_fwd_tc_kernel)"); return LADE_ECUDA; }
   return LADE_OK;
 }
@@ -619,7 +683,7 @@ static int attn_fwd_tc_launch_t(cudaStream_t stream, const void* q, const void* 
                                 int n_heads, int n_kv_heads, int head_dim, int kv_capacity, int kv_bound, int n_splits) {
   (void)kv_bound;
   if (head_dim != TC_D) return LADE_EUNSUPPORTED;
-  if (n_splits > 8) n_splits = 8;   // portable cluster size
+  if (n_splits > 8) n_splits = 8;   // the split count shapes the numerics: same clamp as the cluster-launched impl 3
   return launch_tc<ET, false>(stream, q, k_cache, v_cache, out, rowmask, mask_words, meta, scratch, q_pad, n_heads,
                               n_kv_heads, head_dim, kv_capacity, n_splits);
 }

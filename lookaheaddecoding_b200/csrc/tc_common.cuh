@@ -172,17 +172,6 @@ __device__ __forceinline__ float2 ld_global_f2(const float2* p) {
   asm volatile("ld.global.cg.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
   return v;
 }
-__device__ __forceinline__ void st_dsmem_f4(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-__device__ __forceinline__ void st_dsmem_f2(uint32_t addr, float a, float b) {
-  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
-}
-__device__ __forceinline__ float2 ld_dsmem_f2(uint32_t addr) {
-  float2 v;
-  asm volatile("ld.shared::cluster.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
-  return v;
-}
 
 
 // cuTensorMapEncodeTiled resolved through cudaGetDriverEntryPoint (no libcuda link dependency); null if unavailable.
