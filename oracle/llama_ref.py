@@ -100,6 +100,115 @@ def eager_attention(q, k, v, mask, n_rep: int = 1):
     return torch.matmul(p, v)
 
 
+# ---- float64 attention and its error bound ------------------------------------------------------------------------
+# Constants of the bound (attention_fp64).  Derivation, per output element o[r, d] = sum_j p_j v_jd:
+#   C_ULP = 1:  the final rounding to the model dtype costs <= 0.5 ulp; the other 0.5 ulp covers a result that lands
+#               in the binade above o_ref (its ulp is twice as large) and the fp32 arithmetic of the normalisation.
+#   C_SPREAD = 4:  every probability is rounded to the model dtype once (reference and kernels alike), a relative error
+#               delta_j with |delta_j| <= u_T (absolute <= half the smallest subnormal step below the normal range).
+#               Normalising by the sum of the rounded (impl 2) or unrounded (impl 1) probabilities, or rounding after
+#               the normalisation (impl 3), turns them into sum_j delta_j p_j (v_jd - o_d) or sum_j delta_j p_j v_jd:
+#               a sum of independent, zero-mean errors.  Round-to-nearest of a value with a spread mantissa has an RMS
+#               relative error of about 0.42 u_T, so 4 * u_T * ||p (|v| + |o|)|| is a >= 9 sigma event; even Hoeffding's
+#               inequality, which only uses |delta_j| <= u_T, puts it at <= 2 exp(-8) per element.
+#   SCORE_WINDOW = 2^-20:  the kernels form T(T(raw) * fp32(1/sqrt(D))) with raw summed in fp32, the reference T(T(q.k) /
+#               sqrt(D)).  A score within 2^-20 (relative) of a rounding midpoint of either rounding -- or, for the
+#               first one, within the worst-case fp32 error D * 2^-24 * sum_i |q_i k_i| of the dot product -- may round
+#               the other way; the bound adds what that other rounding does to the output, for those scores only:
+#               p_j (e^Delta_j - 1)(|v_jd| + |o_d|) for a score moved by Delta_j.  That is the whole first-order effect
+#               of the flip, so a flip that happens uses all of it: C_AMB = 2 keeps the margin the other terms have.
+#   the floor:  2^-20 * sum_j p_j |v_jd| for the fp32 accumulation of P.V (<= 24 tile partial sums, each <= 2^-24
+#               relative, plus the split merge), and 2^-100 so that a row that sees nothing (o = 0) divides cleanly.
+C_ULP, C_SPREAD, C_AMB, SCORE_WINDOW = 1.0, 4.0, 2.0, 2.0 ** -20
+_DT_INFO = {torch.bfloat16: (7, -126, 2.0 ** -8, 2.0 ** -134), torch.float16: (10, -14, 2.0 ** -11, 2.0 ** -25)}
+
+
+def ulp(x: torch.Tensor, dtype) -> torch.Tensor:
+    """Spacing of the model dtype `dtype` at |x| (float64), subnormal range included."""
+    mant, emin, _, _ = _DT_INFO[dtype]
+    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** (emin - mant))))
+    return torch.exp2(e.clamp_min(emin) - mant)
+
+
+def _round_alternative(x: torch.Tensor, dtype, window: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(T(x), the other rounding of x where x lies within `window` of the midpoint between T(x) and its neighbour on
+    x's side, else T(x)), both float64."""
+    r = x.to(dtype)
+    rd = r.double()
+    toward = torch.sign(x - rd) * torch.where(rd < 0, -1.0, 1.0)          # +1: step the magnitude up
+    bits = r.view(torch.int16).to(torch.int32) + toward.to(torch.int32)
+    alt = bits.to(torch.int16).view(dtype).double()
+    ambiguous = (toward != 0) & (rd != 0) & ((x - 0.5 * (rd + alt)).abs() <= window) & torch.isfinite(alt)
+    return rd, torch.where(ambiguous, alt, rd)
+
+
+def visibility(step_vis: torch.Tensor, kv_len: int, q_rows: Optional[int] = None) -> torch.Tensor:
+    """[q_rows, kv_len + q_len] bool: every row sees the cache; the step block as given.  Rows past q_len (PAD rows of
+    a fixed-shape step) see the cache and nothing of the step."""
+    q_len = step_vis.shape[0]
+    q_rows = q_len if q_rows is None else q_rows
+    vis = torch.zeros(q_rows, kv_len + q_len, dtype=torch.bool, device=step_vis.device)
+    vis[:, :kv_len] = True
+    vis[:q_len, kv_len:] = step_vis
+    return vis
+
+
+def attention_fp64(q, k, v, vis, dtype) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The reference's attention (modeling_llama.py:520-541) in float64 with the reference's score rounding, and a
+    per-element bound on how far an honest model-dtype kernel may be from it (constants above).
+
+    q [Hq, R, D], k/v [Hkv, T, D] (model dtype values), vis [R, T] bool (or [Hq, R, T]).
+    Returns (o_ref, bound), both float64 [Hq, R, D].  s = T(T(q.k) / sqrt(D)), masked scores are -inf, softmax and P.V
+    in float64; a row that sees nothing gives 0."""
+    _, _, u, eta = _DT_INFO[dtype]
+    Hq, R, D = q.shape
+    n_rep = Hq // k.shape[0]
+    qd = q.double()
+    kd = k.double().repeat_interleave(n_rep, dim=0)
+    vd = v.double().repeat_interleave(n_rep, dim=0)
+    vis = vis.to(q.device).expand(Hq, R, kd.shape[1])
+    raw = qd @ kd.transpose(1, 2)
+    w_raw = torch.maximum(SCORE_WINDOW * raw.abs(), D * 2.0 ** -24 * (qd.abs() @ kd.abs().transpose(1, 2)))
+    r1, r1_alt = _round_alternative(raw, dtype, w_raw)
+    s, s_alt = _round_alternative(r1 / math.sqrt(D), dtype, SCORE_WINDOW * (r1 / math.sqrt(D)).abs())
+    s2, s2_alt = _round_alternative(r1_alt / math.sqrt(D), dtype, SCORE_WINDOW * (r1_alt / math.sqrt(D)).abs())
+    delta = torch.maximum((s_alt - s).abs(), torch.maximum((s2 - s).abs(), (s2_alt - s).abs()))
+    s = s.masked_fill(~vis, -math.inf)
+    m = s.amax(-1, keepdim=True)
+    e = torch.exp(s - torch.where(torch.isfinite(m), m, 0.0))
+    l = e.sum(-1, keepdim=True)
+    p = torch.where(l > 0, e / torch.where(l > 0, l, 1.0), 0.0)
+    o = p @ vd
+    va, oa = vd.abs(), o.abs()
+    # per-probability rounding error: relative u, absolute eta (below the normal range), never more than p itself
+    err_p = torch.minimum(p, torch.maximum(u * p, torch.full_like(p, eta)))
+    err_p = torch.where(vis, err_p, 0.0)
+    e2 = err_p * err_p
+    spread = (e2 @ (vd * vd) + 2 * oa * (e2 @ va) + oa * oa * e2.sum(-1, keepdim=True)).clamp_min(0).sqrt()
+    amb = torch.where(vis, p * torch.expm1(delta), 0.0)
+    amb_term = amb @ va + oa * amb.sum(-1, keepdim=True)
+    bound = C_ULP * ulp(o, dtype) + C_SPREAD * spread + C_AMB * amb_term + 2.0 ** -20 * (p @ va) + 2.0 ** -100
+    return o, bound
+
+
+def bound_ratio(got: torch.Tensor, o_ref: torch.Tensor, bound: torch.Tensor) -> torch.Tensor:
+    """|got - o_ref| / bound, float64 (NaN or inf in `got` gives inf)."""
+    err = (got.double() - o_ref).abs()
+    return torch.where(torch.isfinite(err), err / bound, math.inf)
+
+
+# Acceptance of a kernel output against attention_fp64: no element beyond its bound, and on average well inside it (an
+# honest kernel sits near 0.1; a systematic error such as a 1 % scale moves the mean, not only the tail).
+MAX_RATIO, MEAN_RATIO = 1.0, 0.25
+
+
+def within_bound(got, o_ref, bound) -> Tuple[bool, float, float]:
+    """(passes, max ratio, mean ratio) of `got` against (o_ref, bound) of attention_fp64."""
+    ratio = bound_ratio(got, o_ref, bound)
+    mx, mean = ratio.max().item(), ratio.mean().item()
+    return mx <= MAX_RATIO and mean <= MEAN_RATIO, mx, mean
+
+
 class OracleLlama:
     """Functional Llama with a growing KV cache, driven by ``oracle.lookahead.greedy_lookahead``."""
 

@@ -1,9 +1,12 @@
 """Lookahead attention kernel vs (a) the reference module's own output captured in tests/golden and
-(b) the oracle's restatement of the reference eager attention on seeded inputs.
+(b) the reference attention in float64 (oracle.llama_ref.attention_fp64) on seeded inputs.
 
-Tolerance (bf16 outputs, |o| <~ 1): the kernel keeps the reference's rounding points for the scores but
-uses online softmax (probabilities are rounded to bf16 before normalisation instead of after), so it is
-not bit-identical: max abs error <= 2e-2 and mean abs error <= 2e-3 are required."""
+The kernel keeps the reference's rounding points for the scores but uses online softmax (probabilities are rounded to
+the model dtype before normalisation instead of after), so it is not bit-identical.  Against the float64 reference every
+output element must lie within its own bound -- one ulp of the result, the spread of the probability roundings over the
+row, and the effect of scores that sit on a rounding midpoint -- and on average within a quarter of it (the bound scales
+with the output, so it stays tight at long contexts where the outputs shrink).  The captured module outputs are bf16
+values themselves: those keep an absolute check (max |err| <= 2e-2, mean <= 2e-3)."""
 import os
 
 import numpy as np
@@ -72,6 +75,22 @@ def check_close(got, want):
     assert err.mean().item() <= ATOL_MEAN, f"mean abs err {err.mean().item():.4g}"
 
 
+def check_bound(got, q, k, v, vis, what=""):
+    """got [R, Hq*D] (kernel output rows) against attention_fp64 of q [Hq, R, D], k/v [Hkv, T, D] (valid rows only) and
+    vis [R, T]; prints the worst err/bound."""
+    Hq, R, D = q.shape
+    o_ref, bound = LR.attention_fp64(q.cuda(), k.cuda(), v.cuda(), vis.cuda(), q.dtype)
+    got = got.cuda().view(R, Hq, D).transpose(0, 1)
+    ok, mx, mean = LR.within_bound(got, o_ref, bound)
+    print(f"\n{what} err/bound max {mx:.3f} mean {mean:.3f}")
+    assert ok, f"{what}: err/bound max {mx:.3f} (<= {LR.MAX_RATIO}), mean {mean:.3f} (<= {LR.MEAN_RATIO})"
+    return mx
+
+
+def step_vis(lay, kv_len, rows=None):
+    return LR.visibility(torch.from_numpy(LA.step_mask(lay)), kv_len, rows)
+
+
 @pytest.mark.parametrize("impl", IMPLS)
 @pytest.mark.parametrize("name", ["attn_tiny_bf16_w15n5g15_pool", "attn_gqa_bf16_w15n5g15", "attn_tiny_bf16_w5n3g3"])
 def test_attention_vs_reference_module_output(name, impl):
@@ -90,6 +109,7 @@ def test_attention_vs_reference_module_output(name, impl):
         out = run_kernel(fx["q"].cuda(), fx["k"].cuda(), fx["v"].cuda(), lay, meta_for(lay, kv_len, q_pad),
                          q_pad, n_splits, impl)
         check_close(out.cpu(), fx["o"])
+        check_bound(out, fx["q"], fx["k"], fx["v"], step_vis(lay, kv_len), f"{name} impl {impl} splits {n_splits}")
 
 
 def _oracle_attn(q, k, v, lay, kv_len):
@@ -118,7 +138,7 @@ def test_attention_steady_shapes_vs_oracle(kv_len, W, N, g, Hq, Hkv, splits, imp
     v = torch.randn(Hkv, T, D, device="cuda").to(torch.bfloat16)
     q_pad = gs * (W + max(g, 1)) + 4
     out = run_kernel(q, k, v, lay, meta_for(lay, kv_len, q_pad), q_pad, splits, impl)
-    check_close(out, _oracle_attn(q, k, v, lay, kv_len))
+    check_bound(out, q, k, v, step_vis(lay, kv_len), f"kv {kv_len} impl {impl}")
 
 
 @pytest.mark.parametrize("impl", IMPLS)
@@ -131,7 +151,7 @@ def test_attention_prefill_causal_vs_oracle(P, Hq, Hkv, splits, impl):
     k = torch.randn(Hkv, P, D, device="cuda").to(torch.bfloat16)
     v = torch.randn(Hkv, P, D, device="cuda").to(torch.bfloat16)
     out = run_kernel(q, k, v, lay, meta_for(lay, 0, P), P, splits, impl)
-    check_close(out, _oracle_attn(q, k, v, lay, 0))
+    check_bound(out, q, k, v, torch.ones(P, P, dtype=torch.bool).tril(), f"prefill {P} impl {impl}")
 
 
 @pytest.mark.parametrize("impl", IMPLS)
@@ -150,7 +170,7 @@ def test_attention_lp_shapes_vs_oracle(impl):
         k = torch.randn(Hq, T, 128, device="cuda").to(torch.bfloat16)
         v = torch.randn(Hq, T, 128, device="cuda").to(torch.bfloat16)
         out = run_kernel(q, k, v, lay, meta_for(lay, kv_len, lay.q_len), lay.q_len, 2, impl)
-        check_close(out, _oracle_attn(q, k, v, lay, kv_len))
+        check_bound(out, q, k, v, step_vis(lay, kv_len), f"lp rank {r} impl {impl}")
 
 
 @pytest.mark.parametrize("kv_len,Hq,Hkv,splits", [(0, 4, 4, 1), (77, 4, 2, 3), (700, 8, 2, 4)])
@@ -168,7 +188,7 @@ def test_attention_head_dim_64_vs_oracle(kv_len, Hq, Hkv, splits):
     q_pad = gs * (W + g) + 4
     for impl in (0, 1):
         out = run_kernel(q, k, v, lay, meta_for(lay, kv_len, q_pad), q_pad, splits, impl)
-        check_close(out, _oracle_attn(q, k, v, lay, kv_len))
+        check_bound(out, q, k, v, step_vis(lay, kv_len), f"head_dim 64 kv {kv_len} impl {impl}")
     from lookaheaddecoding_b200 import _cabi
     lib = _cabi.load()
     z = torch.zeros(64, device="cuda")
@@ -180,7 +200,7 @@ def test_attention_head_dim_64_vs_oracle(kv_len, Hq, Hkv, splits):
 @pytest.mark.parametrize("kv_len,D,Hq,Hkv,splits", [(0, 128, 2, 2, 1), (300, 128, 4, 2, 3), (130, 64, 4, 2, 2)])
 def test_attention_fp16_vs_oracle(kv_len, D, Hq, Hkv, splits):
     """fp16 models: lade_attn_fwd_f16 (impl 0: wgmma kernel on fp16 operands for head_dim 128, mma.sync for 64; impl 1:
-    mma.sync) against the reference's eager attention restated in fp16; same absolute tolerance as bf16."""
+    mma.sync) against the float64 reference with fp16 rounding points (u_T = 2^-11 in the bound)."""
     torch.manual_seed(kv_len + D)
     W, N, g = 15, 5, 5
     gs = N - 1
@@ -191,13 +211,10 @@ def test_attention_fp16_vs_oracle(kv_len, D, Hq, Hkv, splits):
     k = torch.randn(Hkv, T, D, device="cuda").to(torch.float16)
     v = torch.randn(Hkv, T, D, device="cuda").to(torch.float16)
     q_pad = gs * (W + g) + 4
-    vis = torch.from_numpy(LA.step_mask(lay)).cuda()
-    mask = LR.additive_mask(vis, kv_len, torch.float16)
-    want = LR.eager_attention(q, k, v, mask, Hq // Hkv).transpose(0, 1).reshape(q_len, -1)
     for impl in (0, 1):
         out = run_kernel(q, k, v, lay, meta_for(lay, kv_len, q_pad), q_pad, splits, impl, dt=torch.float16)
         assert out.dtype == torch.float16
-        check_close(out, want)
+        check_bound(out, q, k, v, step_vis(lay, kv_len), f"fp16 D {D} kv {kv_len} impl {impl}")
 
 
 # ---- impl 3: the wgmma kernel's reference-order variant (probabilities normalised BEFORE they are rounded) ----------
@@ -210,7 +227,7 @@ def _mismatch(a, b):
     (517, 20, 7, 20, 4, 4, 3), (1278, 15, 5, 15, 4, 2, 4), (200, 5, 3, 3, 2, 1, 4),
 ])
 def test_reference_order_variant_rounds_like_the_reference(kv_len, W, N, g, Hq, Hkv, splits):
-    """impl 3 against the restated reference attention: besides the tolerance of the other kernels, (almost) every output
+    """impl 3 against the restated reference attention: besides the bound of the other kernels, (almost) every output
     must be BIT-identical -- what is left is accumulation order (ours: tensor-core tiles and split partials; the
     restatement: cuBLAS) and ex2.approx, a fraction of a percent -- while the online-softmax kernel (impl 2) differs in
     the last bit of about half of them."""
@@ -226,7 +243,7 @@ def test_reference_order_variant_rounds_like_the_reference(kv_len, W, N, g, Hq, 
     want = _oracle_attn(q, k, v, lay, kv_len)
     out3 = run_kernel(q, k, v, lay, meta_for(lay, kv_len, q_pad), q_pad, splits, 3)
     out2 = run_kernel(q, k, v, lay, meta_for(lay, kv_len, q_pad), q_pad, splits, 2)
-    check_close(out3, want)
+    check_bound(out3, q, k, v, step_vis(lay, kv_len), f"impl 3 kv {kv_len}")
     d3, d2 = _mismatch(out3, want), _mismatch(out2, want)
     print(f"\nkv={kv_len} q={q_len}: outputs not bit-identical to the reference math: impl 3 {d3:.4%}, impl 2 {d2:.4%}")
     assert d3 <= 0.02, d3
@@ -243,7 +260,7 @@ def test_reference_order_variant_prefill(P, Hq, Hkv, splits):
     v = torch.randn(Hkv, P, 128, device="cuda").to(torch.bfloat16)
     want = _oracle_attn(q, k, v, lay, 0)
     out = run_kernel(q, k, v, lay, meta_for(lay, 0, P), P, splits, 3)
-    check_close(out, want)
+    check_bound(out, q, k, v, torch.ones(P, P, dtype=torch.bool).tril(), f"impl 3 prefill {P}")
     assert _mismatch(out, want) <= 0.02
 
 
@@ -261,6 +278,7 @@ def test_reference_order_variant_vs_reference_module_output(name):
     for n_splits in (1, 3):
         out = run_kernel(fx["q"].cuda(), fx["k"].cuda(), fx["v"].cuda(), lay, meta_for(lay, kv_len, q_pad), q_pad, n_splits, 3)
         check_close(out.cpu(), fx["o"])
+        check_bound(out, fx["q"], fx["k"], fx["v"], step_vis(lay, kv_len), f"{name} impl 3 splits {n_splits}")
         assert _mismatch(out.cpu(), fx["o"]) <= 0.02
 
 
@@ -278,7 +296,7 @@ def test_reference_order_variant_fp16_and_bounds():
     vis = torch.from_numpy(LA.step_mask(lay)).cuda()
     want = LR.eager_attention(q, k, v, LR.additive_mask(vis, kv_len, torch.float16), Hq // Hkv).transpose(0, 1).reshape(q_len, -1)
     out = run_kernel(q, k, v, lay, meta_for(lay, kv_len, q_pad), q_pad, 3, 3, dt=torch.float16)
-    check_close(out, want)
+    check_bound(out, q, k, v, step_vis(lay, kv_len), "impl 3 fp16")
     assert _mismatch(out, want) <= 0.02
     # more than 3 KV tiles per split do not fit shared memory: refused on the host, loudly (T = 480 rows on one split)
     k2 = torch.randn(Hkv, 400 + q_len, 128, device="cuda").to(torch.float16)
