@@ -65,7 +65,8 @@ __device__ __forceinline__ float score_of(const T* row, int t, float temperature
 // two 256-bin histograms instead of a sort)
 template <typename T>
 __device__ __forceinline__ unsigned key_of(T x) {
-  const unsigned b = Elem<T>::key16(x);
+  unsigned b = Elem<T>::key16(x);
+  if (b == 0x8000u) b = 0u;          // -0 and +0 are one value to the warpers' comparisons: one key
   return (b & 0x8000u) ? (~b & 0xffffu) : (b | 0x8000u);
 }
 
@@ -83,7 +84,7 @@ __device__ __forceinline__ float e_of(const T* row, int t, float temperature, co
 // can go (torch.sort breaks such ties arbitrarily, so there is no reference order to follow inside a bucket).
 template <typename T>
 __device__ RowDist row_dist(const T* row, int vocab, float temperature, int top_k, float top_p, float* s_red,
-                            int* s_cnt, float* s_mass, int* s_sel) {
+                            int* s_cnt, unsigned long long* s_mass, unsigned long long* s_mtot, int* s_sel) {
   RowDist d;
   float mx = -INFINITY;
   unsigned kmax = 0;
@@ -125,37 +126,46 @@ __device__ RowDist row_dist(const T* row, int vocab, float temperature, int top_
     if (key_of(row[t]) >= d.thr) sm += __expf(score_of(row, t, temperature) - d.mx);
   d.sum = block_reduce_sum(sm, s_red);
   if (top_p < 1.f) {
-    const float lim = (1.f - top_p) * d.sum;
+    // Bucket masses in 2^-40 fixed point (every e <= 1, so even 2^17 terms stay below 2^57).  Integer adds are exact:
+    // the cut does not depend on the order of the atomics, and the kept mass total - dropped has no cancellation.
     for (int pass = 0; pass < 2; ++pass) {
-      for (int i = threadIdx.x; i < 256; i += blockDim.x) s_mass[i] = 0.f;
+      for (int i = threadIdx.x; i < 256; i += blockDim.x) s_mass[i] = 0ull;
       __syncthreads();
       const unsigned hb = pass ? (unsigned)s_sel[0] : 0u;
       for (int t = threadIdx.x; t < vocab; t += blockDim.x) {
         const unsigned k = key_of(row[t]);
         if (k < d.thr) continue;
-        const float e = __expf(score_of(row, t, temperature) - d.mx);
+        const unsigned long long e = __float2ull_rn(__expf(score_of(row, t, temperature) - d.mx) * 0x1p40f);
         if (pass == 0) atomicAdd(&s_mass[k >> 8], e);
         else if ((k >> 8) == hb) atomicAdd(&s_mass[k & 255u], e);
       }
       __syncthreads();
       if (threadIdx.x == 0) {
-        float cum = pass ? s_red[0] : 0.f;                   // mass of the buckets already dropped (s_red[0]: scratch)
+        if (pass == 0) {
+          unsigned long long total = 0;
+          for (int b = 0; b < 256; ++b) total += s_mass[b];
+          s_mtot[0] = total;
+          s_mtot[1] = 0;                                     // mass of the buckets already dropped
+        }
+        const double lim = (1.0 - (double)top_p) * (double)s_mtot[0];
+        unsigned long long cum = s_mtot[1];
+        // min_tokens_to_keep = 1: the scan stops at the bucket of the largest key at the latest
+        const int last = pass ? ((top_key >> 8) == hb ? (int)(top_key & 255u) : 255) : (int)(top_key >> 8);
         int b = 0;
-        for (; b < 255; ++b) {
-          if (!(cum + s_mass[b] <= lim)) break;              // this bucket crosses 1 - top_p: it stays
+        for (; b < last; ++b) {
+          if (!((double)(cum + s_mass[b]) <= lim)) break;    // this bucket crosses 1 - top_p: it stays
           cum += s_mass[b];
         }
         if (pass == 0) s_sel[0] = b;
         else s_sel[2] = b;
-        s_red[0] = cum;
+        s_mtot[1] = cum;
       }
       __syncthreads();
     }
-    unsigned thr_p = ((unsigned)s_sel[0] << 8) | (unsigned)s_sel[2];
-    const float dropped = s_red[0];
+    const unsigned thr_p = ((unsigned)s_sel[0] << 8) | (unsigned)s_sel[2];
+    const unsigned long long kept = s_mtot[0] - s_mtot[1];
     __syncthreads();
-    if (thr_p > top_key) thr_p = top_key;                    // min_tokens_to_keep = 1
-    if (thr_p > d.thr) { d.thr = thr_p; d.sum -= dropped; }
+    if (thr_p > d.thr) { d.thr = thr_p; d.sum = (float)((double)kept * 0x1p-40); }
   }
   if (d.thr > top_key) d.thr = top_key;
   return d;
@@ -232,7 +242,8 @@ sample_verify_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int 
                      unsigned long long* rng_state, int* __restrict__ rec, float* dbg) {
   __shared__ float s_red[32];
   __shared__ int s_cnt[256];
-  __shared__ float s_mass[256];
+  __shared__ unsigned long long s_mass[256];
+  __shared__ unsigned long long s_mtot[2];
   __shared__ int s_sel[4];
   __shared__ float s_scan[SMP_THREADS];
   __shared__ int s_pick;
@@ -267,7 +278,7 @@ sample_verify_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int 
 
   const T* row0 = logits;                       // slot 0 = the next-token row (lade_step_layout's lm_rows)
   if (phase != 2 || n_ng == 0) {                // :458-480, :543-546
-    const RowDist rs = row_dist(row0, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_sel);
+    const RowDist rs = row_dist(row0, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_mtot, s_sel);
     if (t == 0) s_u = draw();
     __syncthreads();
     const int tok = multinomial_excluding(row0, vocab, temperature, rs, s_u, s_z, 0, s_scan, &s_pick);
@@ -279,7 +290,7 @@ sample_verify_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int 
     for (int i = 0; i < GS; ++i) {
       const int cur = s_ctl[1];
       const T* row = logits + (long long)cur * ld;
-      const RowDist rs = row_dist(row, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_sel);
+      const RowDist rs = row_dist(row, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_mtot, s_sel);
       if (t == 0) {
         int n_z = 0;
         float zmass = 0.f;                      // probability mass rejected so far at this position
