@@ -98,6 +98,28 @@ typedef struct LadeConfig {
   int32_t rank;             /* LOCAL_RANK                                             */
 } LadeConfig;
 
+/* Greedy logits processors applied on device by lade_argmax_processed (HF transformers 5.5,
+ * generation/logits_process.py).  The reference forbids any processor on its greedy path (lade/decoding.py:968);
+ * greedy lookahead stays lossless under a processor that depends only on the prefix a row stands for, which is what
+ * these three do.  One record per generate() call, written to device memory by lade_processors_upload. */
+enum {
+  LADE_PROC_REPETITION_PENALTY = 1, /* RepetitionPenaltyLogitsProcessor(penalty, prompt_ignore_length)           */
+  LADE_PROC_NO_REPEAT_NGRAM = 2,    /* NoRepeatNGramLogitsProcessor(ngram_size)                                  */
+  LADE_PROC_MIN_LENGTH = 4,         /* MinLengthLogitsProcessor / MinNewTokensLengthLogitsProcessor              */
+  LADE_PROC_MAX_NGRAM = 64,
+  LADE_PROC_MAX_EOS = 8
+};
+typedef struct LadeProcessors {
+  int32_t flags;                  /* LADE_PROC_* bits of the active processors                                */
+  uint32_t penalty_bits;          /* fp32 bits of the repetition penalty (> 0, finite)                        */
+  int32_t prompt_ignore_length;   /* the penalty acts on prefix[prompt_ignore_length:]                       */
+  int32_t ngram_size;             /* 1 .. LADE_PROC_MAX_NGRAM                                                 */
+  int32_t eos_bound;              /* eos ids score -inf while the prefix is shorter: max(min_length,
+                                     prompt_length_to_skip + min_new_tokens)                                  */
+  int32_t n_eos;                  /* 0 .. LADE_PROC_MAX_EOS                                                   */
+  int32_t eos_token_id[8];
+} LadeProcessors;
+
 /* ---- context --------------------------------------------------------------------------------- */
 
 /* Allocates the device-resident decode state (window, n-gram pool, token buffers).
@@ -236,6 +258,24 @@ int lade_sample_verify_f16(LadeCtx* ctx, void* stream, const void* logits, int32
  * (torch.argmax at lade/decoding.py:1021,1041,1052,1072,1102). */
 int lade_argmax_rows(void* stream, const void* logits, int32_t n_rows, int32_t vocab, int32_t ld,
                      int32_t* out_idx);
+
+/* lade_argmax_rows under the greedy logits processors of `proc_dev` (device LadeProcessors): every lm slot is scored
+ * as HF's greedy _sample scores the position it stands for, argmax(processors(prefix, fp32(logits[slot]))), lowest
+ * index on ties.  Prefix of slot 0: the committed ids out_ids[0, n_out); of verification slot 1+(W+N-3)+i (i below the
+ * step's guess-token count; n-gram e = i / (N-1), position u = i % (N-1)): the committed ids followed by the n-gram's
+ * tokens 0..u.  Window slots are plain argmax.  Lifts the reference's "no logits processors" restriction
+ * (lade/decoding.py:968) for RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor, MinLengthLogitsProcessor
+ * and MinNewTokensLengthLogitsProcessor.  Reads n_out, the guess count and the guess tokens from the ctx state, so it
+ * runs after lade_step_layout of the same step.  LADE_EUNSUPPORTED for vocab > 163840 (shared-memory bitmaps) or a
+ * lookahead-parallel ctx.  With no flag set the output equals lade_argmax_rows. */
+int lade_argmax_processed(LadeCtx* ctx, void* stream, const void* logits, int32_t n_rows, int32_t vocab, int32_t ld,
+                          const LadeProcessors* proc_dev, int32_t* out_idx);
+int lade_argmax_processed_f16(LadeCtx* ctx, void* stream, const void* logits, int32_t n_rows, int32_t vocab, int32_t ld,
+                              const LadeProcessors* proc_dev, int32_t* out_idx);
+/* Validate a host LadeProcessors record and copy it to `dev` on `stream` (stream-ordered; the host record may be
+ * reused on return).  LADE_EINVAL for unknown flags, a penalty that is not finite and > 0, a negative
+ * prompt_ignore_length, ngram_size outside 1..LADE_PROC_MAX_NGRAM, or more than LADE_PROC_MAX_EOS eos ids. */
+int lade_processors_upload(void* stream, const LadeProcessors* host, LadeProcessors* dev);
 
 /* Verification + state update of one step, fully on device: longest-prefix accept
  * (lade/decoding.py:1071-1084), window fill / shift (:1038-1066,:1119-1124), n-gram pool LRU update

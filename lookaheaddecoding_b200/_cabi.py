@@ -31,6 +31,17 @@ class LadeConfig(C.Structure):
     ]
 
 
+PROC_REPETITION_PENALTY, PROC_NO_REPEAT_NGRAM, PROC_MIN_LENGTH = 1, 2, 4
+PROC_MAX_NGRAM, PROC_MAX_EOS = 64, 8
+
+
+class LadeProcessors(C.Structure):
+    _fields_ = [
+        ("flags", c_i32), ("penalty_bits", C.c_uint32), ("prompt_ignore_length", c_i32), ("ngram_size", c_i32),
+        ("eos_bound", c_i32), ("n_eos", c_i32), ("eos_token_id", c_i32 * PROC_MAX_EOS),
+    ]
+
+
 class LadeError(RuntimeError):
     pass
 
@@ -52,6 +63,8 @@ _SIGNATURES = {
     "lade_debug_gemm_timing": (C.c_int, [c_p]),
     "lade_swiglu": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32]),
     "lade_argmax_rows": (C.c_int, [c_p, c_p, c_i32, c_i32, c_i32, c_p]),
+    "lade_argmax_processed": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32, c_i32, c_p, c_p]),
+    "lade_processors_upload": (C.c_int, [c_p, C.POINTER(LadeProcessors), c_p]),
     "lade_accept_update": (C.c_int, [c_p, c_p, c_p, c_p, c_p]),
     "lade_commit_decision": (C.c_int, [c_p, c_p, c_p, c_p, c_p]),
     "lade_sample_verify": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32, c_p, c_p, C.c_float, c_i32, C.c_float, c_p, c_p, c_p]),
@@ -74,7 +87,7 @@ _SIGNATURES = {
 
 # fp16 twins: same signatures as the bf16 entry points
 for _name in ("lade_rmsnorm", "lade_rmsnorm_gather", "lade_rope_append", "lade_swiglu", "lade_argmax_rows", "lade_attn_fwd",
-              "lade_sample_verify"):
+              "lade_sample_verify", "lade_argmax_processed"):
     _SIGNATURES[_name + "_f16"] = _SIGNATURES[_name]
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

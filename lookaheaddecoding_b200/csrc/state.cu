@@ -11,6 +11,7 @@
 //   emission / EOS / stopping       lade/decoding.py:1165-1177, :1205-1219
 #include "state.cuh"
 
+#include <cstring>
 #include <new>
 #include <string>
 
@@ -563,9 +564,17 @@ __global__ void kv_compact_kernel(const int* __restrict__ res, __nv_bfloat16* k_
 }
 
 // ---- row-wise argmax (lowest index on ties) ------------------------------------------------------------
-template <typename T>
-__global__ void argmax_rows_kernel(const T* __restrict__ logits, int vocab, int ld, int* out_idx) {
-  const int row = blockIdx.x;
+// Argmax of row `row` into out_idx[row], by the whole CTA: 16-byte loads when the row is aligned, each element converted
+// to fp32 and passed through `score(f, id)` (the identity for lade_argmax_rows, the logits processors for
+// lade_argmax_processed) before it competes, then a lowest-index reduction over the block.  An all -inf row yields 0,
+// like torch.argmax.
+struct IdentityScore {
+  __device__ __forceinline__ float operator()(float f, int) const { return f; }
+};
+
+template <typename T, typename Score>
+__device__ __forceinline__ void argmax_row(const T* __restrict__ logits, int vocab, int ld, int row, Score score,
+                                           int* out_idx) {
   const T* p = logits + (long long)row * ld;
   float best = -INFINITY;
   int bi = 0x7fffffff;
@@ -579,18 +588,18 @@ __global__ void argmax_rows_kernel(const T* __restrict__ logits, int vocab, int 
       const T* e = reinterpret_cast<const T*>(&v);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const float f = Elem<T>::to_f(e[j]);
+        const float f = score(Elem<T>::to_f(e[j]), i * 8 + j);
         const int id = i * 8 + j;
         if (f > best || (f == best && id < bi)) { best = f; bi = id; }
       }
     }
     for (int id = nvec * 8 + t; id < vocab; id += blockDim.x) {
-      const float f = Elem<T>::to_f(p[id]);
+      const float f = score(Elem<T>::to_f(p[id]), id);
       if (f > best || (f == best && id < bi)) { best = f; bi = id; }
     }
   } else {
     for (int id = t; id < vocab; id += blockDim.x) {
-      const float f = Elem<T>::to_f(p[id]);
+      const float f = score(Elem<T>::to_f(p[id]), id);
       if (f > best || (f == best && id < bi)) { best = f; bi = id; }
     }
   }
@@ -618,6 +627,108 @@ __global__ void argmax_rows_kernel(const T* __restrict__ logits, int vocab, int 
     }
     if (lane == 0) out_idx[row] = (bi == 0x7fffffff) ? 0 : bi;
   }
+}
+
+template <typename T>
+__global__ void argmax_rows_kernel(const T* __restrict__ logits, int vocab, int ld, int* out_idx) {
+  argmax_row(logits, vocab, ld, blockIdx.x, IdentityScore(), out_idx);
+}
+
+// ---- argmax under the greedy logits processors ----------------------------------------------------------
+// Slot s of the lm rows is scored as HF's greedy step scores the position it stands for:
+// argmax(processors(prefix, fp32(logits[s]))).  Prefix of slot 0: out_ids[0, n_out); of verification slot 1+WCAP+i
+// (i < lg, n-gram e = i / GS, position u = i % GS): out_ids[0, n_out) + guess[e*GS .. e*GS+u] -- the columns row_sees
+// gives that GUESS row.  Window slots (and verification slots past lg, which accept never reads) stay plain argmax.
+// Each CTA marks its prefix's tokens in two V-bit shared bitmaps, "penalised" (RepetitionPenaltyLogitsProcessor) and
+// "banned" (NoRepeatNGramLogitsProcessor's n-gram matches, the eos ids of MinLength / MinNewTokensLength while the
+// prefix is shorter than eos_bound), then scores the row in one pass.  Ban and penalty commute (a banned score is
+// -inf either way), so the result does not depend on the order HF lists the processors in.
+struct ProcessedScore {
+  const unsigned* pen;
+  const unsigned* ban;
+  float pf, inv;
+  bool rep;
+  __device__ __forceinline__ float operator()(float f, int id) const {
+    const unsigned m = 1u << (id & 31);
+    const int w = id >> 5;
+    // torch on CUDA: `score * penalty` with the penalty cast to fp32, `score / penalty` as score * fp32(1 / penalty)
+    if (rep && (pen[w] & m)) f = f < 0.f ? __fmul_rn(f, pf) : __fmul_rn(f, inv);
+    return (ban[w] & m) ? -INFINITY : f;
+  }
+};
+
+template <typename T>
+__global__ void __launch_bounds__(256) argmax_processed_kernel(const T* __restrict__ logits, int vocab, int ld,
+                                                               const int* __restrict__ st, Dims d,
+                                                               const LadeProcessors* __restrict__ proc, int* out_idx) {
+  extern __shared__ unsigned s_bits[];          // [words] penalised, then [words] banned
+  const int slot = blockIdx.x;
+  const int t = threadIdx.x;
+  const int flags = proc->flags;
+  const int n_out = st[S_N_OUT];
+  const int lg = st[S_N_GUESS_TOK];
+  int len = -1, g0 = 0;
+  if (slot == 0) {
+    len = n_out;
+  } else if (slot >= 1 + d.WCAP && slot - 1 - d.WCAP < lg) {
+    const int i = slot - 1 - d.WCAP;
+    const int u = i % d.GS;
+    g0 = i - u;
+    len = n_out + u + 1;
+  }
+  if (len < 0 || flags == 0) {
+    argmax_row(logits, vocab, ld, slot, IdentityScore(), out_idx);
+    return;
+  }
+  const int words = (vocab + 31) >> 5;
+  unsigned* pen = s_bits;
+  unsigned* ban = s_bits + words;
+  for (int w = t; w < 2 * words; w += blockDim.x) s_bits[w] = 0u;
+  __syncthreads();
+  const int* out = st + d.off_out;
+  const int* gs = st + d.off_guess + g0;
+  auto tok = [&](int k) { return k < n_out ? out[k] : gs[k - n_out]; };
+  auto mark = [&](unsigned* bits, int id) {
+    if (id >= 0 && id < vocab) atomicOr(bits + (id >> 5), 1u << (id & 31));
+  };
+  const bool rep = (flags & LADE_PROC_REPETITION_PENALTY) != 0;
+  if (rep)
+    for (int k = max(proc->prompt_ignore_length, 0) + t; k < len; k += blockDim.x) mark(pen, tok(k));
+  if (flags & LADE_PROC_NO_REPEAT_NGRAM) {
+    // the n-gram starting at j bans its last token when its first n-1 tokens equal the prefix's last n-1
+    // (_calc_banned_ngram_tokens; nothing while len + 1 < n, and n = 1 bans every prefix token)
+    const int n = proc->ngram_size;
+    if (n >= 1 && n <= LADE_PROC_MAX_NGRAM) {
+      const int tail = len - n + 1;
+      for (int j = t; j <= len - n; j += blockDim.x) {
+        bool match = true;
+        for (int q = 0; q < n - 1 && match; ++q) match = tok(j + q) == tok(tail + q);
+        if (match) mark(ban, tok(j + n - 1));
+      }
+    }
+  }
+  if ((flags & LADE_PROC_MIN_LENGTH) && len < proc->eos_bound && t < min(max(proc->n_eos, 0), LADE_PROC_MAX_EOS))
+    mark(ban, proc->eos_token_id[t]);
+  __syncthreads();
+  const float pf = __uint_as_float(proc->penalty_bits);
+  ProcessedScore score{pen, ban, pf, __frcp_rn(pf), rep};
+  argmax_row(logits, vocab, ld, slot, score, out_idx);
+}
+
+// Bitmaps of lade_argmax_processed: two of ceil(vocab / 32) words in dynamic shared memory, kept within the 48 KB a
+// launch gets without opting in.
+static const int kProcMaxVocab = 160 * 1024;
+
+template <typename T>
+static int launch_argmax_processed(LadeCtx* ctx, void* stream, const void* logits, int32_t n_rows, int32_t vocab,
+                                   int32_t ld, const LadeProcessors* proc_dev, int32_t* out_idx) {
+  if (!ctx || !logits || !proc_dev || !out_idx || n_rows < 1 || vocab < 1 || ld < vocab) return LADE_EINVAL;
+  if (vocab > kProcMaxVocab || ctx->d.D != 1) return LADE_EUNSUPPORTED;
+  const size_t smem = sizeof(unsigned) * 2 * (size_t)((vocab + 31) / 32);
+  argmax_processed_kernel<T><<<n_rows, 256, smem, (cudaStream_t)stream>>>((const T*)logits, vocab, ld, ctx->state,
+                                                                          ctx->d, proc_dev, out_idx);
+  LADE_LAUNCH_CHECK("argmax_processed_kernel");
+  return LADE_OK;
 }
 
 static int make_dims(const LadeConfig& c, Dims* d) {
@@ -771,6 +882,33 @@ int lade_argmax_rows_f16(void* stream, const void* logits, int32_t n_rows, int32
   return LADE_OK;
 }
 
+int lade_argmax_processed(LadeCtx* ctx, void* stream, const void* logits, int32_t n_rows, int32_t vocab, int32_t ld,
+                          const LadeProcessors* proc_dev, int32_t* out_idx) {
+  return launch_argmax_processed<__nv_bfloat16>(ctx, stream, logits, n_rows, vocab, ld, proc_dev, out_idx);
+}
+
+int lade_argmax_processed_f16(LadeCtx* ctx, void* stream, const void* logits, int32_t n_rows, int32_t vocab,
+                              int32_t ld, const LadeProcessors* proc_dev, int32_t* out_idx) {
+  return launch_argmax_processed<__half>(ctx, stream, logits, n_rows, vocab, ld, proc_dev, out_idx);
+}
+
+int lade_processors_upload(void* stream, const LadeProcessors* host, LadeProcessors* dev) {
+  if (!host || !dev) return LADE_EINVAL;
+  const int known = LADE_PROC_REPETITION_PENALTY | LADE_PROC_NO_REPEAT_NGRAM | LADE_PROC_MIN_LENGTH;
+  if (host->flags & ~known) return LADE_EINVAL;
+  if (host->flags & LADE_PROC_REPETITION_PENALTY) {
+    uint32_t b = host->penalty_bits;
+    float pf;
+    memcpy(&pf, &b, sizeof(pf));
+    if (!(pf > 0.f) || !(pf < INFINITY) || host->prompt_ignore_length < 0) return LADE_EINVAL;
+  }
+  if ((host->flags & LADE_PROC_NO_REPEAT_NGRAM) && (host->ngram_size < 1 || host->ngram_size > LADE_PROC_MAX_NGRAM))
+    return LADE_EINVAL;
+  if (host->n_eos < 0 || host->n_eos > LADE_PROC_MAX_EOS) return LADE_EINVAL;
+  LADE_CUDA_CHECK(cudaMemcpyAsync(dev, host, sizeof(LadeProcessors), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  return LADE_OK;
+}
+
 int lade_ctx_output_ids(LadeCtx* ctx, void* stream, int32_t* out_host, int32_t n) {
   if (!ctx || !out_host || n < 0 || n > ctx->d.cap) return LADE_EINVAL;
   LADE_CUDA_CHECK(cudaMemcpyAsync(out_host, ctx->state + ctx->d.off_out, sizeof(int32_t) * n,
@@ -842,6 +980,6 @@ const char* lade_strerror(int code) {
 
 const char* lade_last_cuda_error(void) { return lade::g_last_error.c_str(); }
 
-int lade_version(void) { return 101; }
+int lade_version(void) { return 102; }
 
 }  // extern "C"

@@ -107,6 +107,43 @@ def _host_stop_fn(extra, device, dtype):
     return stop
 
 
+def processors_from_hf(logits_processor) -> Optional[dict]:
+    """The engine's `processors` dict for a greedy LogitsProcessorList, read from the processors' own attributes.  Only
+    processors that depend on nothing but the row's prefix are supported: RepetitionPenaltyLogitsProcessor,
+    NoRepeatNGramLogitsProcessor, MinLengthLogitsProcessor and MinNewTokensLengthLogitsProcessor (the reference allows
+    none, lade/decoding.py:968).  Anything else raises a LadeError naming its class."""
+    from transformers.generation.logits_process import (MinLengthLogitsProcessor, MinNewTokensLengthLogitsProcessor,
+                                                        NoRepeatNGramLogitsProcessor, RepetitionPenaltyLogitsProcessor)
+    if not logits_processor:
+        return None
+    out, bounds, eos = {}, [], None
+    for p in logits_processor:
+        kind = type(p)
+        if kind in (RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor) and \
+                ("penalty" if kind is RepetitionPenaltyLogitsProcessor else "ngram_size") in out:
+            raise LadeError(f"{kind.__name__} given twice: not supported on the lookahead greedy path")
+        if kind is RepetitionPenaltyLogitsProcessor:
+            out["penalty"] = float(p.penalty)
+            out["prompt_ignore_length"] = int(p.prompt_ignore_length or 0)
+        elif kind is NoRepeatNGramLogitsProcessor:
+            out["ngram_size"] = int(p.ngram_size)
+        elif kind in (MinLengthLogitsProcessor, MinNewTokensLengthLogitsProcessor):
+            ids = sorted({int(e) for e in torch.as_tensor(p.eos_token_id).reshape(-1).tolist()})
+            if eos is not None and ids != eos:
+                raise LadeError("the min-length logits processors name different eos ids: not supported")
+            eos = ids
+            bounds.append(int(p.min_length) if kind is MinLengthLogitsProcessor
+                          else int(p.prompt_length_to_skip) + int(p.min_new_tokens))
+        else:
+            raise LadeError(f"logits processor {kind.__name__} is not supported on the lookahead greedy path "
+                            "(supported: RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor, "
+                            "MinLengthLogitsProcessor, MinNewTokensLengthLogitsProcessor)")
+    if bounds:
+        out["min_length"] = max(bounds)
+        out["eos_token_id"] = eos
+    return out
+
+
 def get_engine(model, **overrides) -> LookaheadEngine:
     """One engine per (model, lookahead config); reads CONFIG_MAP like lade/decoding.py:854-862."""
     W = CONFIG_MAP.get("WINDOW_SIZE", 60)
@@ -144,15 +181,17 @@ def jacobi_greedy_search_multilevel(self, input_ids: torch.LongTensor, logits_pr
                                     chat: bool = False, stop_token: Optional[str] = None, **model_kwargs):
     """Greedy lookahead decoding on the H100 engine; drop-in for lade/decoding.py:697-1259.
 
-    Inherited restrictions (fail loudly, as the reference asserts): batch size 1
-    (modeling_llama.py:1448), no logits processors (:968), ``return_dict_in_generate == False``
+    Logits processors: the prefix-only ones of ``processors_from_hf`` run on device (the reference allows none,
+    :968); any other raises.  Inherited restrictions (fail loudly, as the reference asserts): batch size 1
+    (modeling_llama.py:1448), ``return_dict_in_generate == False``
     (:967), ``ALWAYS_FWD_ONE == 1`` (:873), LEVEL >= 3 (:902).  ``stop_token`` / ``chat`` are
     accepted and ignored (UI only).
     """
     if input_ids.shape[0] != 1:
         raise LadeError("lookahead decoding supports batch size 1 only (modeling_llama.py:1448)")
-    if logits_processor is not None and len(logits_processor) != 0:
-        raise LadeError("logits processors are not supported on the lookahead greedy path (decoding.py:968)")
+    processors = processors_from_hf(logits_processor)
+    if processors and CONFIG_MAP.get("DIST_WORKERS", 1) > 1:
+        raise LadeError("logits processors are not supported with lookahead parallelism (DIST_WORKERS > 1)")
     if return_dict_in_generate:
         raise LadeError("return_dict_in_generate must be False (decoding.py:967)")
     if CONFIG_MAP.get("ALWAYS_FWD_ONE", 1) != 1:
@@ -170,7 +209,8 @@ def jacobi_greedy_search_multilevel(self, input_ids: torch.LongTensor, logits_pr
     eng = get_engine(self, max_total_len=total, min_total_len=total)
     prompt = input_ids[0].tolist()
     stop_fn = _host_stop_fn(_extra_stopping_criteria(stopping_criteria), input_ids.device, input_ids.dtype)
-    out = eng.generate(prompt, total - init_len, eos_token_ids=eos_token_id or (), rng=random, stop_fn=stop_fn)
+    out = eng.generate(prompt, total - init_len, eos_token_ids=eos_token_id or (), rng=random, stop_fn=stop_fn,
+                       processors=processors)
     if streamer is not None:
         streamer.put(torch.tensor(out[init_len:]))
         streamer.end()

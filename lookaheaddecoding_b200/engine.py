@@ -46,6 +46,43 @@ def _ptr(t: Optional[torch.Tensor]) -> int:
     return 0 if t is None else t.data_ptr()
 
 
+_PROC_KEYS = ("penalty", "prompt_ignore_length", "ngram_size", "min_length", "eos_token_id")
+
+
+def processors_record(processors: dict) -> _cabi.LadeProcessors:
+    """The LadeProcessors record of a `processors` dict (see LookaheadEngine.generate).  The penalty is rounded to fp32
+    as torch does for a python scalar on a float32 tensor."""
+    unknown = set(processors) - set(_PROC_KEYS)
+    if unknown:
+        raise LadeError(f"unknown logits-processor fields {sorted(unknown)} (known: {', '.join(_PROC_KEYS)})")
+    r = _cabi.LadeProcessors()
+    if processors.get("penalty") is not None:
+        p = np.float32(processors["penalty"])
+        if not (np.isfinite(p) and p > 0):
+            raise LadeError(f"repetition penalty must be finite and > 0 (got {processors['penalty']})")
+        r.flags |= _cabi.PROC_REPETITION_PENALTY
+        r.penalty_bits = int(p.view(np.uint32))
+        r.prompt_ignore_length = int(processors.get("prompt_ignore_length") or 0)
+        if r.prompt_ignore_length < 0:
+            raise LadeError("prompt_ignore_length must be >= 0")
+    if processors.get("ngram_size") is not None:
+        n = int(processors["ngram_size"])
+        if not 1 <= n <= _cabi.PROC_MAX_NGRAM:
+            raise LadeError(f"no_repeat_ngram_size must be in 1..{_cabi.PROC_MAX_NGRAM} on device (got {n})")
+        r.flags |= _cabi.PROC_NO_REPEAT_NGRAM
+        r.ngram_size = n
+    eos = [int(e) for e in (processors.get("eos_token_id") or ())]
+    if processors.get("min_length") is not None and eos:
+        if len(eos) > _cabi.PROC_MAX_EOS:
+            raise LadeError(f"at most {_cabi.PROC_MAX_EOS} eos ids for the min-length processors (got {len(eos)})")
+        r.flags |= _cabi.PROC_MIN_LENGTH
+        r.eos_bound = int(processors["min_length"])
+        r.n_eos = len(eos)
+        for i, e in enumerate(eos):
+            r.eos_token_id[i] = e
+    return r
+
+
 class LookaheadEngine:
     """Device-resident lookahead decoding for one Llama model (batch 1, bf16, CUDA)."""
 
@@ -69,6 +106,7 @@ class LookaheadEngine:
         self.k_rope_append = getattr(self.lib, "lade_rope_append" + sfx)
         self.k_swiglu = getattr(self.lib, "lade_swiglu" + sfx)
         self.k_argmax_rows = getattr(self.lib, "lade_argmax_rows" + sfx)
+        self.k_argmax_processed = getattr(self.lib, "lade_argmax_processed" + sfx)
         self.k_attn_fwd = getattr(self.lib, "lade_attn_fwd" + sfx)
         self.k_sample_verify = getattr(self.lib, "lade_sample_verify" + sfx)
         if level < 3:
@@ -155,6 +193,9 @@ class LookaheadEngine:
         # two result slots + events: the host reads step i's record while step i+1 is already queued on the GPU
         self._pinned_ring = [torch.empty(_cabi.RES_INTS, dtype=torch.int32, pin_memory=True) for _ in range(2)]
         self._res_events = [torch.cuda.Event() for _ in range(2)]
+        # greedy logits processors of the current generate() (LadeProcessors, written by begin()); off: plain argmax
+        self.proc_dev = torch.zeros(C.sizeof(_cabi.LadeProcessors) // 4, dtype=torch.int32, device=self.dev)
+        self.processors_on = False
         self.launches = 0   # kernels of THIS repo launched (graph replays counted by their content)
         # tests set a device float[>= 2 + G*(N-1) + W]: lade_sample_verify then records the uniforms it consumed
         self.debug_uniforms: Optional[torch.Tensor] = None
@@ -330,8 +371,13 @@ class LookaheadEngine:
         check(self.k_rmsnorm_gather(stream, _ptr(h), _ptr(delta), _ptr(self.norm_w), _ptr(self.lm_rows),
                                       _ptr(self.xn_lm), self.lm_cap, self.H, self.eps), "lade_rmsnorm_gather"); n += 1
         n += self._proj(self.xn_lm, self.lm_head, self.logits)
-        check(self.k_argmax_rows(stream, _ptr(self.logits), self.lm_cap, self.V, self.V, _ptr(self.am)),
-              "lade_argmax_rows"); n += 1
+        if self.processors_on:
+            check(self.k_argmax_processed(self._ctx, stream, _ptr(self.logits), self.lm_cap, self.V, self.V,
+                                          _ptr(self.proc_dev), _ptr(self.am)), "lade_argmax_processed")
+        else:
+            check(self.k_argmax_rows(stream, _ptr(self.logits), self.lm_cap, self.V, self.V, _ptr(self.am)),
+                  "lade_argmax_rows")
+        n += 1
         return n + self._commit(stream, commit)
 
     def _norm(self, stream: int, h, delta, w, out, rows: int) -> int:
@@ -458,7 +504,7 @@ class LookaheadEngine:
         if self._graph is None:
             self._graph = {}
         key = (commit, float(self.sample_temperature), int(self.sample_top_k), float(self.sample_top_p)) \
-            if commit == "sample" else commit
+            if commit == "sample" else (commit, self.processors_on)
         if key in self._graph:
             self._graph_n = self._graph[key][1]
             return self._graph[key][0]
@@ -489,11 +535,16 @@ class LookaheadEngine:
             self._steady_graph(commit).replay()
             self.launches += self._graph_n
 
-    def begin(self, prompt, max_length: int, eos_token_ids, window0) -> None:
-        """Reset the device state for a generate() call (lade_ctx_reset) and size the buffers."""
+    def begin(self, prompt, max_length: int, eos_token_ids, window0, processors: Optional[dict] = None) -> None:
+        """Reset the device state for a generate() call (lade_ctx_reset), write the logits-processor record and size
+        the buffers."""
         P = len(prompt)
+        rec = processors_record(processors) if processors else None
         self._ensure_ctx(eos_token_ids)
         stream = torch.cuda.current_stream(self.dev).cuda_stream
+        if rec is not None:
+            check(self.lib.lade_processors_upload(stream, C.byref(rec), _ptr(self.proc_dev)), "lade_processors_upload")
+        self.processors_on = rec is not None
         prompt_np = np.asarray(prompt, dtype=np.int32)
         win_np = np.asarray(list(window0), dtype=np.int32)
         check(self.lib.lade_ctx_reset(self._ctx, stream, prompt_np.ctypes.data, P, win_np.ctypes.data, len(win_np),
@@ -522,19 +573,28 @@ class LookaheadEngine:
     @torch.no_grad()
     def generate(self, prompt_ids: Sequence[int], max_new_tokens: int, eos_token_ids: Sequence[int] = (),
                  rng: Optional[random.Random] = None, window0: Optional[Sequence[int]] = None,
-                 stop_fn=None, sampling: Optional[dict] = None) -> List[int]:
+                 stop_fn=None, sampling: Optional[dict] = None, processors: Optional[dict] = None) -> List[int]:
         """Greedy lookahead decoding; returns prompt + generated ids (trimmed to P + max_new_tokens).
         `stop_fn(ids) -> bool`: host-evaluated stopping criteria beyond max-length / EOS, checked after every step
         like lade/decoding.py:1215 (disables the one-step-deep host pipelining).
         `sampling={"temperature": T, "top_k": k, "top_p": p, "seed": s}`: the sampling loop (jacobi_sample_multilevel, lade/decoding.py:137) with
         the verification on device (lade_sample_verify, Philox stream seeded by `s`): same host loop, same CUDA graph
-        replay per step, the only difference is the commit kernels at the end of the step."""
+        replay per step, the only difference is the commit kernels at the end of the step.
+        `processors={"penalty": p, "prompt_ignore_length": k, "ngram_size": n, "min_length": m, "eos_token_id": [...]}`
+        (every key optional): HF's greedy RepetitionPenalty / NoRepeatNGram / MinLength logits processors, applied on
+        device to every row the step's verification reads, each against the prefix that row stands for
+        (lade_argmax_processed).  "min_length" is the length below which the eos ids score -inf
+        (max(min_length, prompt_length + min_new_tokens) for HF's two processors).  Greedy and one GPU only."""
         prompt = [int(t) for t in prompt_ids]
         P = len(prompt)
         max_length = P + int(max_new_tokens)
         if max_length > self.max_total_len:
             raise LadeError(f"prompt+max_new_tokens={max_length} exceeds engine capacity {self.max_total_len}")
         commit = True
+        if processors and sampling is not None:
+            raise LadeError("logits processors are supported on the greedy path only (not with sampling=)")
+        if processors and self.DW != 1:
+            raise LadeError("logits processors are not supported with lookahead parallelism (DIST_WORKERS > 1)")
         if sampling is not None:
             if self.DW != 1:
                 raise LadeError("the sampling path has no lookahead parallelism (reference: replicas only)")
@@ -546,7 +606,7 @@ class LookaheadEngine:
                 raise LadeError("top_k must be >= 0 and top_p in (0, 1]")
             self.sample_temperature, self.sample_top_k, self.sample_top_p = T, top_k, top_p
             commit = "sample"
-        self.begin(prompt, max_length, eos_token_ids, self.draw_window(prompt, rng, window0))
+        self.begin(prompt, max_length, eos_token_ids, self.draw_window(prompt, rng, window0), processors)
         if sampling is not None:
             self.rng_state.copy_(torch.tensor([int(sampling.get("seed", 0)) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64))
         stream = torch.cuda.current_stream(self.dev).cuda_stream
