@@ -120,6 +120,20 @@ typedef struct LadeProcessors {
   int32_t eos_token_id[8];
 } LadeProcessors;
 
+/* Sampling warpers of lade_sample_verify_warped, in HF's list order (transformers 5.5,
+ * GenerationMixin._get_logits_processor): TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper ->
+ * MinPLogitsWarper -> EpsilonLogitsWarper -> EtaLogitsWarper, every one with min_tokens_to_keep = 1 and filter value
+ * -inf.  top_k = 0, top_p = 1 and 0 for the last three switch a warper off. */
+typedef struct LadeWarpers {
+  float temperature;   /* > 0                                                                         */
+  int32_t top_k;       /* >= 0                                                                        */
+  float top_p;         /* (0, 1]                                                                      */
+  float min_p;         /* [0, 1]: drop probs < min_p * max(probs)                    (MinPLogitsWarper) */
+  float epsilon;       /* 0 or (0, 1): drop probs < epsilon, never the maximum    (EpsilonLogitsWarper) */
+  float eta;           /* 0 or (0, 1): drop probs < min(eta, sqrt(eta) * exp(-entropy)), never the maximum
+                          (EtaLogitsWarper)                                                           */
+} LadeWarpers;
+
 /* ---- context --------------------------------------------------------------------------------- */
 
 /* Allocates the device-resident decode state (window, n-gram pool, token buffers).
@@ -301,6 +315,28 @@ int lade_accept_update(LadeCtx* ctx, void* stream, const int32_t* argmax_slots, 
 int lade_sample_verify(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab,
                        const int32_t* argmax_slots, const int32_t* meta, float temperature, int32_t top_k, float top_p,
                        uint64_t* rng_state, int32_t* decision_out, float* debug_uniforms);
+
+/* lade_sample_verify under the full warper record `warpers` (host memory, read at launch: a captured graph keeps the
+ * values of its capture).  After top-p, every row the verification visits -- slot 0 and the row after each accepted
+ * token -- is cut further, each warper acting on the softmax of what the previous ones kept (logits_process.py):
+ *   MinPLogitsWarper     probs = softmax(scores); remove probs < min_p * probs.amax()
+ *                        (with e_t = exp(score_t - max): e_t < min_p);
+ *   EpsilonLogitsWarper  remove softmax(scores) < epsilon & scores < topk(scores, 1);
+ *   EtaLogitsWarper      entropy = Categorical(logits=scores).entropy(); eta = min(epsilon, sqrt(epsilon) * exp(-entropy));
+ *                        remove softmax(scores) < eta & scores < topk(scores, 1).
+ * Each kept set is every score at or above a threshold, so each cut is one more threshold on the key (one pass over
+ * the vocabulary; eta one more for the entropy), evaluated in fp32; the accept tests, the residual and the plain draw
+ * use e_t / S' with S' summed over the final kept set.  The cuts consume no random numbers: the Philox stream and its
+ * advance are those of lade_sample_verify, and with the three cuts off the decision is bit for bit the same.
+ * `debug_cuts` (nullable, device float[>= 1 + 2 (N-1)]): [rows visited, then per row its final threshold key (the
+ * 16-bit order key of the smallest kept logit) and S'], for tests.  LADE_EINVAL for min_p outside [0, 1], epsilon or
+ * eta outside {0} or (0, 1), any NaN, or the temperature / top_k / top_p ranges of lade_sample_verify. */
+int lade_sample_verify_warped(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab,
+                              const int32_t* argmax_slots, const int32_t* meta, const LadeWarpers* warpers,
+                              uint64_t* rng_state, int32_t* decision_out, float* debug_uniforms, float* debug_cuts);
+int lade_sample_verify_warped_f16(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab,
+                                  const int32_t* argmax_slots, const int32_t* meta, const LadeWarpers* warpers,
+                                  uint64_t* rng_state, int32_t* decision_out, float* debug_uniforms, float* debug_cuts);
 
 /* Apply an externally made decision (sampling path: the caller runs the reference's rejection-sampling
  * verification, lade/decoding.py:484-540, against the device logits with its own RNG streams).

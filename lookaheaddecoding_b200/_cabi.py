@@ -42,6 +42,11 @@ class LadeProcessors(C.Structure):
     ]
 
 
+class LadeWarpers(C.Structure):
+    _fields_ = [("temperature", C.c_float), ("top_k", c_i32), ("top_p", C.c_float), ("min_p", C.c_float),
+                ("epsilon", C.c_float), ("eta", C.c_float)]
+
+
 class LadeError(RuntimeError):
     pass
 
@@ -68,6 +73,8 @@ _SIGNATURES = {
     "lade_accept_update": (C.c_int, [c_p, c_p, c_p, c_p, c_p]),
     "lade_commit_decision": (C.c_int, [c_p, c_p, c_p, c_p, c_p]),
     "lade_sample_verify": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32, c_p, c_p, C.c_float, c_i32, C.c_float, c_p, c_p, c_p]),
+    "lade_sample_verify_warped": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32, c_p, c_p, C.POINTER(LadeWarpers), c_p, c_p, c_p,
+                                            c_p]),
     "lade_kv_compact": (C.c_int, [c_p, c_p, c_p, c_p, C.c_int64, c_i32, c_i32, c_i32, c_i32, c_i32]),
     "lade_ctx_output_ids": (C.c_int, [c_p, c_p, c_p, c_i32]),
     "lade_ctx_pool_snapshot": (C.c_int, [c_p, c_p, c_p, c_p]),
@@ -87,7 +94,7 @@ _SIGNATURES = {
 
 # fp16 twins: same signatures as the bf16 entry points
 for _name in ("lade_rmsnorm", "lade_rmsnorm_gather", "lade_rope_append", "lade_swiglu", "lade_argmax_rows", "lade_attn_fwd",
-              "lade_sample_verify", "lade_argmax_processed"):
+              "lade_sample_verify", "lade_argmax_processed", "lade_sample_verify_warped"):
     _SIGNATURES[_name + "_f16"] = _SIGNATURES[_name]
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

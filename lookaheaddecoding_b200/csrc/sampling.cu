@@ -171,6 +171,88 @@ __device__ RowDist row_dist(const T* row, int vocab, float temperature, int top_
   return d;
 }
 
+// Cut-offs of the three threshold warpers after top-p (0 = off; the C-ABI has checked the ranges).
+struct Warpers { float min_p, epsilon, eta; };
+
+// Smallest key among the kept tokens (key >= thr) that pass `keep`; thr itself when none does.  Every warper below
+// keeps the top token, so the result never exceeds the top key.
+template <typename T, typename Keep>
+__device__ __forceinline__ unsigned min_kept_key(const T* row, int vocab, unsigned thr, Keep keep, float* s_red) {
+  float best = -65536.f;                                     // max of -key: 16-bit keys are exact in fp32
+  for (int t = threadIdx.x; t < vocab; t += blockDim.x) {
+    const unsigned k = key_of(row[t]);
+    if (k >= thr && keep(t)) best = fmaxf(best, -(float)k);
+  }
+  const float r = -block_reduce_max(best, s_red);
+  return r > 65535.f ? thr : (unsigned)r;
+}
+
+// (S, sum of e_t x_t) over the kept tokens, x_t = score_t - mx, e_t = exp(x_t): the mass and the entropy term.
+template <typename T>
+__device__ __forceinline__ float2 kept_moments(const T* row, int vocab, float temperature, const RowDist& d,
+                                               float* s_red) {
+  float sm = 0.f, sx = 0.f;
+  for (int t = threadIdx.x; t < vocab; t += blockDim.x) {
+    if (key_of(row[t]) < d.thr) continue;
+    const float x = score_of(row, t, temperature) - d.mx;
+    const float e = __expf(x);
+    sm += e;
+    if (e > 0.f) sx += e * x;                                // an underflowed term adds nothing (and no -inf * 0)
+  }
+  return make_float2(block_reduce_sum(sm, s_red), block_reduce_sum(sx, s_red));
+}
+
+// row_dist followed by MinPLogitsWarper -> EpsilonLogitsWarper -> EtaLogitsWarper (HF's list order; each acts on the
+// softmax of what the previous ones kept; min_tokens_to_keep = 1, filter value -inf).  With p_t = e_t / S:
+// * MinP drops p_t < min_p * max p, i.e. e_t < min_p (the top token's e is 1);
+// * Epsilon drops p_t < epsilon unless the score is the maximum;
+// * Eta drops p_t < min(eta, sqrt(eta) exp(-H)), H = ln S - sum(e_t x_t) / S the entropy of the kept distribution,
+//   again unless the score is the maximum.
+// A cut is a threshold on the key (the score is monotone in it), so each is one more pass for the smallest key that
+// stays, and the kept set stays an upper set of the key.  d.sum is recomputed over the final kept set whenever a cut
+// moved the threshold (the top-p kept mass no longer applies then).  `wdbg` (nullable): per visited row, the final
+// threshold key and S'.
+template <typename T>
+__device__ RowDist row_dist_warped(const T* row, int vocab, float temperature, int top_k, float top_p, const Warpers& w,
+                                   float* s_red, int* s_cnt, unsigned long long* s_mass, unsigned long long* s_mtot,
+                                   int* s_sel, float* wdbg) {
+  RowDist d = row_dist(row, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_mtot, s_sel);
+  bool stale = false;                                        // d.sum is not the mass of the current kept set
+  if (w.min_p > 0.f) {
+    const float mp = w.min_p;
+    const unsigned thr = min_kept_key(row, vocab, d.thr, [&](int t) {
+      return __expf(score_of(row, t, temperature) - d.mx) >= mp; }, s_red);
+    if (thr > d.thr) { d.thr = thr; stale = true; }
+  }
+  if (w.epsilon > 0.f) {
+    if (stale) { d.sum = kept_moments(row, vocab, temperature, d, s_red).x; stale = false; }
+    const float eps = w.epsilon, S = d.sum;
+    const unsigned thr = min_kept_key(row, vocab, d.thr, [&](int t) {
+      const float s = score_of(row, t, temperature);
+      return s == d.mx || !(__expf(s - d.mx) / S < eps); }, s_red);
+    if (thr > d.thr) { d.thr = thr; stale = true; }
+  }
+  if (w.eta > 0.f) {
+    const float2 m = kept_moments(row, vocab, temperature, d, s_red);
+    d.sum = m.x;
+    stale = false;
+    const float ent = logf(m.x) - m.y / m.x;
+    const float eta = fminf(w.eta, sqrtf(w.eta) * expf(-ent)), S = d.sum;
+    const unsigned thr = min_kept_key(row, vocab, d.thr, [&](int t) {
+      const float s = score_of(row, t, temperature);
+      return s == d.mx || !(__expf(s - d.mx) / S < eta); }, s_red);
+    if (thr > d.thr) { d.thr = thr; stale = true; }
+  }
+  if (stale) d.sum = kept_moments(row, vocab, temperature, d, s_red).x;
+  if (wdbg && threadIdx.x == 0) {
+    const int n = (int)wdbg[0];
+    wdbg[1 + 2 * n] = (float)d.thr;
+    wdbg[2 + 2 * n] = d.sum;
+    wdbg[0] = (float)(n + 1);
+  }
+  return d;
+}
+
 // One draw from the distribution e_t = exp(score_t - mx) over t not in zset[0..n_z), by inverse CDF:
 // the smallest t whose running mass reaches u * total.  Each thread owns one contiguous chunk of the vocabulary.
 template <typename T>
@@ -235,11 +317,13 @@ __device__ int multinomial_excluding(const T* row, int vocab, float temperature,
 // decision_out: the record lade_commit_decision consumes --
 //   [first hit, max_hit, n_new, hits[GS], new_tok[WCAP] | max_hit_idx, flags (1 sampling, 2 filtered row present),
 //    finished-by-extra-eos, 0, filtered[W]]
-template <typename T>
-__global__ void __launch_bounds__(SMP_THREADS, 1)
-sample_verify_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int vocab,
-                     const int* __restrict__ am, const int* __restrict__ meta, float temperature, int top_k, float top_p,
-                     unsigned long long* rng_state, int* __restrict__ rec, float* dbg) {
+// The whole verification of one step; WARPED adds the cuts of row_dist_warped to every row the chain visits.
+template <typename T, bool WARPED>
+__device__ __forceinline__ void sample_verify_chain(int* st, const Dims& d, const T* __restrict__ logits, int ld, int vocab,
+                                                    const int* __restrict__ am, const int* __restrict__ meta,
+                                                    float temperature, int top_k, float top_p, const Warpers& wp,
+                                                    unsigned long long* rng_state, int* __restrict__ rec, float* dbg,
+                                                    float* wdbg) {
   __shared__ float s_red[32];
   __shared__ int s_cnt[256];
   __shared__ unsigned long long s_mass[256];
@@ -278,7 +362,10 @@ sample_verify_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int 
 
   const T* row0 = logits;                       // slot 0 = the next-token row (lade_step_layout's lm_rows)
   if (phase != 2 || n_ng == 0) {                // :458-480, :543-546
-    const RowDist rs = row_dist(row0, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_mtot, s_sel);
+    RowDist rs;
+    if constexpr (WARPED) rs = row_dist_warped(row0, vocab, temperature, top_k, top_p, wp, s_red, s_cnt, s_mass, s_mtot,
+                                               s_sel, wdbg);
+    else rs = row_dist(row0, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_mtot, s_sel);
     if (t == 0) s_u = draw();
     __syncthreads();
     const int tok = multinomial_excluding(row0, vocab, temperature, rs, s_u, s_z, 0, s_scan, &s_pick);
@@ -290,7 +377,10 @@ sample_verify_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int 
     for (int i = 0; i < GS; ++i) {
       const int cur = s_ctl[1];
       const T* row = logits + (long long)cur * ld;
-      const RowDist rs = row_dist(row, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_mtot, s_sel);
+      RowDist rs;
+      if constexpr (WARPED) rs = row_dist_warped(row, vocab, temperature, top_k, top_p, wp, s_red, s_cnt, s_mass, s_mtot,
+                                                 s_sel, wdbg);
+      else rs = row_dist(row, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_mtot, s_sel);
       if (t == 0) {
         int n_z = 0;
         float zmass = 0.f;                      // probability mass rejected so far at this position
@@ -374,6 +464,27 @@ sample_verify_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int 
   }
 }
 
+template <typename T>
+__global__ void __launch_bounds__(SMP_THREADS, 1)
+sample_verify_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int vocab,
+                     const int* __restrict__ am, const int* __restrict__ meta, float temperature, int top_k, float top_p,
+                     unsigned long long* rng_state, int* __restrict__ rec, float* dbg) {
+  sample_verify_chain<T, false>(st, d, logits, ld, vocab, am, meta, temperature, top_k, top_p, Warpers{0.f, 0.f, 0.f},
+                                rng_state, rec, dbg, nullptr);
+}
+
+// sample_verify_kernel with MinP / Epsilon / Eta after top-p.  wdbg (nullable): [rows visited, (thr, S') per row].
+template <typename T>
+__global__ void __launch_bounds__(SMP_THREADS, 1)
+sample_verify_warped_kernel(int* st, Dims d, const T* __restrict__ logits, int ld, int vocab,
+                            const int* __restrict__ am, const int* __restrict__ meta, float temperature, int top_k,
+                            float top_p, Warpers wp, unsigned long long* rng_state, int* __restrict__ rec, float* dbg,
+                            float* wdbg) {
+  if (wdbg && threadIdx.x == 0) wdbg[0] = 0.f;
+  sample_verify_chain<T, true>(st, d, logits, ld, vocab, am, meta, temperature, top_k, top_p, wp, rng_state, rec, dbg,
+                               wdbg);
+}
+
 }  // namespace lade
 
 using namespace lade;
@@ -393,6 +504,30 @@ static int sample_verify_impl(LadeCtx* ctx, void* stream, const void* logits, in
   return LADE_OK;
 }
 
+// MinP / epsilon / eta ranges of HF's constructors (0 = off); NaN fails every comparison
+static bool warpers_valid(const LadeWarpers& w) {
+  const bool cut_ok = (w.min_p >= 0.f && w.min_p <= 1.f) && (w.epsilon == 0.f || (w.epsilon > 0.f && w.epsilon < 1.f)) &&
+                      (w.eta == 0.f || (w.eta > 0.f && w.eta < 1.f));
+  return cut_ok && w.temperature > 0.f && w.top_k >= 0 && w.top_p > 0.f && w.top_p <= 1.f;
+}
+
+template <typename T>
+static int sample_verify_warped_impl(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab,
+                                     const int32_t* argmax_slots, const int32_t* meta, const LadeWarpers* w,
+                                     uint64_t* rng_state, int32_t* decision_out, float* debug_uniforms,
+                                     float* debug_cuts) {
+  if (!ctx || !logits || !argmax_slots || !meta || !w || !rng_state || !decision_out) return LADE_EINVAL;
+  if (!warpers_valid(*w) || vocab < 1 || ld < vocab) return LADE_EINVAL;
+  if (ctx->d.D != 1) return LADE_ESTATE;
+  if (ctx->d.G > SMP_MAX_NGRAMS || ctx->d.GS > 64) return LADE_EUNSUPPORTED;
+  sample_verify_warped_kernel<T><<<1, SMP_THREADS, 0, (cudaStream_t)stream>>>(
+      ctx->state, ctx->d, (const T*)logits, ld, vocab, argmax_slots, meta, w->temperature, w->top_k, w->top_p,
+      Warpers{w->min_p, w->epsilon, w->eta}, reinterpret_cast<unsigned long long*>(rng_state), decision_out,
+      debug_uniforms, debug_cuts);
+  LADE_LAUNCH_CHECK("sample_verify_warped_kernel");
+  return LADE_OK;
+}
+
 extern "C" {
 
 int lade_sample_verify(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab,
@@ -407,6 +542,20 @@ int lade_sample_verify_f16(LadeCtx* ctx, void* stream, const void* logits, int32
                            uint64_t* rng_state, int32_t* decision_out, float* debug_uniforms) {
   return sample_verify_impl<__half>(ctx, stream, logits, ld, vocab, argmax_slots, meta, temperature, top_k, top_p,
                                     rng_state, decision_out, debug_uniforms);
+}
+
+int lade_sample_verify_warped(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab,
+                              const int32_t* argmax_slots, const int32_t* meta, const LadeWarpers* warpers,
+                              uint64_t* rng_state, int32_t* decision_out, float* debug_uniforms, float* debug_cuts) {
+  return sample_verify_warped_impl<__nv_bfloat16>(ctx, stream, logits, ld, vocab, argmax_slots, meta, warpers, rng_state,
+                                                  decision_out, debug_uniforms, debug_cuts);
+}
+
+int lade_sample_verify_warped_f16(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab,
+                                  const int32_t* argmax_slots, const int32_t* meta, const LadeWarpers* warpers,
+                                  uint64_t* rng_state, int32_t* decision_out, float* debug_uniforms, float* debug_cuts) {
+  return sample_verify_warped_impl<__half>(ctx, stream, logits, ld, vocab, argmax_slots, meta, warpers, rng_state,
+                                           decision_out, debug_uniforms, debug_cuts);
 }
 
 }  // extern "C"

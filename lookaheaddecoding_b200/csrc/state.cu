@@ -980,6 +980,6 @@ const char* lade_strerror(int code) {
 
 const char* lade_last_cuda_error(void) { return lade::g_last_error.c_str(); }
 
-int lade_version(void) { return 102; }
+int lade_version(void) { return 103; }
 
 }  // extern "C"

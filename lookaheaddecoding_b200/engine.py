@@ -109,6 +109,7 @@ class LookaheadEngine:
         self.k_argmax_processed = getattr(self.lib, "lade_argmax_processed" + sfx)
         self.k_attn_fwd = getattr(self.lib, "lade_attn_fwd" + sfx)
         self.k_sample_verify = getattr(self.lib, "lade_sample_verify" + sfx)
+        self.k_sample_verify_warped = getattr(self.lib, "lade_sample_verify_warped" + sfx)
         if level < 3:
             raise LadeError("LEVEL must be >= 3 (lade/decoding.py:902)")
         if guess_set_size == -1:
@@ -199,6 +200,8 @@ class LookaheadEngine:
         self.launches = 0   # kernels of THIS repo launched (graph replays counted by their content)
         # tests set a device float[>= 2 + G*(N-1) + W]: lade_sample_verify then records the uniforms it consumed
         self.debug_uniforms: Optional[torch.Tensor] = None
+        # tests set a device float[>= 1 + 2*(N-1)]: lade_sample_verify_warped then records each visited row's cut
+        self.debug_cuts: Optional[torch.Tensor] = None
         self.last_steps = 0
         self.last_records: List[StepRecord] = []
 
@@ -275,6 +278,7 @@ class LookaheadEngine:
         if not hasattr(self, "rng_state"):
             self.rng_state = torch.zeros(2, dtype=torch.int64, device=dev)     # Philox (seed, offset), advanced on device
             self.sample_temperature, self.sample_top_k, self.sample_top_p = 1.0, 0, 1.0
+            self.sample_min_p, self.sample_epsilon, self.sample_eta = 0.0, 0.0, 0.0
         self.lp_send = torch.zeros(self.rec_ints, **i32)
         self.lp_recv = torch.zeros(self.DW * self.rec_ints, **i32)
         self.h = torch.empty(rows, self.H, dtype=bf, device=dev)
@@ -421,7 +425,17 @@ class LookaheadEngine:
         lib = self.lib
         if not commit:
             return 0
-        if commit == "sample":
+        if commit == "sample" and self._cuts_on():
+            w = _cabi.LadeWarpers(float(self.sample_temperature), int(self.sample_top_k), float(self.sample_top_p),
+                                  float(self.sample_min_p), float(self.sample_epsilon), float(self.sample_eta))
+            check(self.k_sample_verify_warped(self._ctx, stream, _ptr(self.logits), self.V, self.V, _ptr(self.am),
+                                              _ptr(self.meta), C.byref(w), _ptr(self.rng_state), _ptr(self.dec_dev),
+                                              _ptr(self.debug_uniforms), _ptr(self.debug_cuts)),
+                  "lade_sample_verify_warped")
+            check(lib.lade_commit_decision(self._ctx, stream, _ptr(self.dec_dev), _ptr(self.meta), _ptr(self.res)),
+                  "lade_commit_decision")
+            n = 2
+        elif commit == "sample":
             check(self.k_sample_verify(self._ctx, stream, _ptr(self.logits), self.V, self.V, _ptr(self.am), _ptr(self.meta),
                                        float(self.sample_temperature), int(self.sample_top_k), float(self.sample_top_p),
                                        _ptr(self.rng_state), _ptr(self.dec_dev), _ptr(self.debug_uniforms)),
@@ -441,6 +455,10 @@ class LookaheadEngine:
                                   self.kv.stride(0), self.L, self.nkv, self.kv_capacity, self.D, max(self.GS - 1, 1)),
               "lade_kv_compact")
         return n + 1
+
+    def _cuts_on(self) -> bool:
+        """Any of MinP / epsilon / eta set: the sampling step runs lade_sample_verify_warped."""
+        return bool(self.sample_min_p or self.sample_epsilon or self.sample_eta)
 
     def _lp_comm_create(self) -> None:
         """In-library NCCL communicator for the per-step record exchange (lade_lp_exchange): rank 0 draws the unique
@@ -503,7 +521,8 @@ class LookaheadEngine:
     def _steady_graph(self, commit: bool = True):
         if self._graph is None:
             self._graph = {}
-        key = (commit, float(self.sample_temperature), int(self.sample_top_k), float(self.sample_top_p)) \
+        key = (commit, float(self.sample_temperature), int(self.sample_top_k), float(self.sample_top_p),
+               float(self.sample_min_p), float(self.sample_epsilon), float(self.sample_eta)) \
             if commit == "sample" else (commit, self.processors_on)
         if key in self._graph:
             self._graph_n = self._graph[key][1]
@@ -579,7 +598,9 @@ class LookaheadEngine:
         like lade/decoding.py:1215 (disables the one-step-deep host pipelining).
         `sampling={"temperature": T, "top_k": k, "top_p": p, "seed": s}`: the sampling loop (jacobi_sample_multilevel, lade/decoding.py:137) with
         the verification on device (lade_sample_verify, Philox stream seeded by `s`): same host loop, same CUDA graph
-        replay per step, the only difference is the commit kernels at the end of the step.
+        replay per step, the only difference is the commit kernels at the end of the step.  Optional further keys
+        "min_p" ([0, 1]), "epsilon" and "eta" (0 or (0, 1)): HF's MinP / Epsilon / Eta warpers after top-p, 0 = off
+        (lade_sample_verify_warped when any is on).
         `processors={"penalty": p, "prompt_ignore_length": k, "ngram_size": n, "min_length": m, "eos_token_id": [...]}`
         (every key optional): HF's greedy RepetitionPenalty / NoRepeatNGram / MinLength logits processors, applied on
         device to every row the step's verification reads, each against the prefix that row stands for
@@ -604,7 +625,14 @@ class LookaheadEngine:
             top_k, top_p = int(sampling.get("top_k", 0) or 0), float(sampling.get("top_p", 1.0))
             if top_k < 0 or not 0.0 < top_p <= 1.0:
                 raise LadeError("top_k must be >= 0 and top_p in (0, 1]")
+            cuts = [float(sampling.get(k, 0.0) or 0.0) for k in ("min_p", "epsilon", "eta")]
+            if not 0.0 <= cuts[0] <= 1.0:
+                raise LadeError(f"min_p must be in [0, 1] (got {sampling.get('min_p')})")
+            for name, v in zip(("epsilon", "eta"), cuts[1:]):
+                if not (v == 0.0 or 0.0 < v < 1.0):
+                    raise LadeError(f"{name} must be 0 (off) or in (0, 1) (got {v})")
             self.sample_temperature, self.sample_top_k, self.sample_top_p = T, top_k, top_p
+            self.sample_min_p, self.sample_epsilon, self.sample_eta = cuts
             commit = "sample"
         self.begin(prompt, max_length, eos_token_ids, self.draw_window(prompt, rng, window0), processors)
         if sampling is not None:

@@ -2,8 +2,9 @@
 
 Two ways to run the multi-candidate rejection-sampling verification (``decoding.py:484-540``, modified SpecInfer):
 
-* **device (default for the warper lists HF builds from temperature / top_k / top_p)**: ``lade_sample_verify`` --
-  temperature, top-k and top-p cut-offs, softmax, accept tests, zero-and-renormalise, residual multinomial draw and
+* **device (default for the warper lists HF builds from temperature / top_k / top_p / min_p / epsilon_cutoff /
+  eta_cutoff)**: ``lade_sample_verify`` (``lade_sample_verify_warped`` with min_p, epsilon or eta) --
+  temperature, top-k, top-p, min-p, epsilon and eta cut-offs, softmax, accept tests, zero-and-renormalise, residual multinomial draw and
   the EOS window filter in one kernel driven by a Philox stream -- followed by ``lade_commit_decision``; the whole step replays from one CUDA graph and the host loop is the
   pipelined greedy loop (``LookaheadEngine.generate(..., sampling=...)``).  Same distribution as the reference, its own
   random stream (seeded from torch's global generator, so ``torch.manual_seed`` makes a run reproducible).
@@ -13,8 +14,9 @@ Two ways to run the multi-candidate rejection-sampling verification (``decoding.
   ``random.random()`` for the accept tests and ``torch.multinomial`` for the residual draw in the reference's order,
   so that under fixed seeds the token stream follows the reference draw for draw (the fixed-seed golden tests).
 
-Restrictions inherited from the reference: warpers within {Temperature, TopK, TopP} (``decoding.py:375-377``),
-no other logits processors (``:412``), batch 1, ``return_dict_in_generate == False``; no lookahead
+Restrictions inherited from the reference: warpers within {Temperature, TopK, TopP} (``decoding.py:375-377``), to
+which this port adds the threshold warpers {MinP, Epsilon, Eta} (each keeps every score at or above a cut, so lookahead
+stays lossless: every verification row is warped as its own distribution, like the top-p cut); no other logits processors (``:412``), batch 1, ``return_dict_in_generate == False``; no lookahead
 parallelism on this path (the reference has none either beyond the initial window broadcast).
 """
 from __future__ import annotations
@@ -30,20 +32,28 @@ from . import _cabi
 from ._cabi import LadeError, check
 
 
+def _supported_warpers():
+    """The warper classes of the sampling path, in HF's list order (GenerationMixin._get_logits_processor)."""
+    from transformers.generation.logits_process import (EpsilonLogitsWarper, EtaLogitsWarper, MinPLogitsWarper,
+                                                        TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper)
+    return (TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper, MinPLogitsWarper, EpsilonLogitsWarper,
+            EtaLogitsWarper)
+
+
 def split_warpers(logits_processor):
     """transformers 5.x keeps the warpers inside the processor list; split them back out."""
-    from transformers.generation.logits_process import (LogitsProcessorList, TemperatureLogitsWarper,
-                                                        TopKLogitsWarper, TopPLogitsWarper)
+    from transformers.generation.logits_process import LogitsProcessorList
+    supported = _supported_warpers()
     procs, warpers = LogitsProcessorList(), LogitsProcessorList()
     for p in (logits_processor or []):
-        (warpers if isinstance(p, (TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper)) else procs).append(p)
+        (warpers if isinstance(p, supported) else procs).append(p)
     return procs, warpers
 
 
 def _check_warpers(logits_warper):
-    from transformers.generation.logits_process import TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper
+    supported = _supported_warpers()
     for w in (logits_warper or []):
-        if type(w) not in (TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper):
+        if type(w) not in supported:
             raise LadeError(f"please set top_k=0.0 and top_p=1.0 {w}")                     # decoding.py:377
 
 
@@ -71,6 +81,32 @@ def device_sampling_params(logits_warper):
     if not T > 0 or k < 0 or not 0.0 < p <= 1.0:
         return None
     return T, k, p
+
+
+def device_warper_params(logits_warper):
+    """dict(temperature, top_k, top_p, min_p, epsilon, eta) -- the LadeWarpers record -- when the warper list is what HF
+    builds from generate(temperature=, top_k=, top_p=, min_p=, epsilon_cutoff=, eta_cutoff=): each warper at most once,
+    in HF's order, -inf filter value, min_tokens_to_keep = 1; else None (host-RNG compatibility loop).  Values are read
+    from the warpers' own attributes (EtaLogitsWarper holds its epsilon as an fp32 tensor)."""
+    supported = _supported_warpers()
+    rank_of = {cls: r for r, cls in enumerate(supported)}
+    names = ("temperature", "top_k", "top_p", "min_p", "epsilon", "eta")
+    attrs = ("temperature", "top_k", "top_p", "min_p", "epsilon", "epsilon")      # each warper's own attribute
+    out = dict(temperature=1.0, top_k=0, top_p=1.0, min_p=0.0, epsilon=0.0, eta=0.0)
+    last = -1
+    for w in list(logits_warper or []):
+        rank = rank_of.get(type(w))
+        if rank is None or rank <= last:
+            return None
+        last = rank
+        if rank > 0 and (getattr(w, "filter_value", -float("inf")) != -float("inf")
+                         or getattr(w, "min_tokens_to_keep", 1) != 1):
+            return None
+        value = getattr(w, attrs[rank])
+        out[names[rank]] = int(value) if rank == 1 else float(value.item() if torch.is_tensor(value) else value)
+    ok = (out["temperature"] > 0 and out["top_k"] >= 0 and 0.0 < out["top_p"] <= 1.0 and 0.0 <= out["min_p"] <= 1.0
+          and all(out[k] == 0.0 or 0.0 < out[k] < 1.0 for k in ("epsilon", "eta")))
+    return out if ok else None
 
 
 def device_temperature(logits_warper):
@@ -235,12 +271,11 @@ def jacobi_sample_multilevel(self, input_ids: torch.LongTensor, logits_processor
             CONFIG_MAP["DIST_WORKERS"] = saved
     from .decoding import _extra_stopping_criteria, _host_stop_fn
     stop_fn = _host_stop_fn(_extra_stopping_criteria(stopping_criteria), input_ids.device, input_ids.dtype)
-    params = device_sampling_params(logits_warper)
+    params = device_warper_params(logits_warper)
     if params is not None and not CONFIG_MAP.get("SAMPLING_ON_HOST", 0):
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # reproducible under torch.manual_seed
         out = eng.generate(input_ids[0].tolist(), total - init_len, eos_token_ids=eos_token_id or (), rng=random,
-                           stop_fn=stop_fn, sampling={"temperature": params[0], "top_k": params[1], "top_p": params[2],
-                                                      "seed": seed})
+                           stop_fn=stop_fn, sampling=dict(params, seed=seed))
     else:
         out = sample_lookahead(eng, input_ids[0].tolist(), total - init_len, logits_warper, eos_token_id or (), rng=random,
                                stop_fn=stop_fn)
