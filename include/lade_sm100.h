@@ -232,7 +232,16 @@ int lade_debug_attn_pdl(int32_t enable);
  * for step row counts m <= 128; `a_rows` >= m is the number of addressable rows of the `a` buffer (rows >= m
  * are read but never stored).  tile_n / split_k = 0 lets the library pick (one wave of CTAs over the SMs);
  * tuning knobs ride in tile_n: bits [16,20) = pipeline depth cap, bit 20 = do not prefill the ring during CTA set-up.
- * Returns LADE_EUNSUPPORTED for m > 128, k % 64 != 0 or n % 8 != 0 (callers then use a library GEMM). */
+ * Returns LADE_EUNSUPPORTED for m > 128, k % 64 != 0 or n % 8 != 0 (callers then use a library GEMM), and for
+ * m < 1, a_rows < m, n < 1, k < 1, ldc < n or ldc % 8 != 0; LADE_EINVAL for a, w or c not 16-byte aligned.
+ * Forced configurations (the low 16 bits of tile_n, or split_k, non-zero; a zero split_k is then 1, a zero tile the
+ * library's choice) launch nothing and return LADE_EINVAL unless all of these hold:
+ *   tile is a multiple of 32 in [32, 256]; split_k is 1, 2, 4 or 8 and divides the k / 64 k-blocks;
+ *   with split_k > 1 the fp32 staging tile of the split reduction fits the pipeline ring it reuses:
+ *     128 * (tile + 4) * 4 <= stages * (16384 + 128 * tile)  bytes, where
+ *     stages = min(floor(231232 / (16384 + 128 * tile)), 11, k / 64 / split_k, depth cap if given).
+ * Rows [m, a_rows) of `a` may hold anything, NaN included: output rows are independent and only rows < m and columns
+ * < n of `c` are written, whatever ldc is. */
 int lade_gemm_bf16(void* stream, const void* a, const void* w, void* c, int32_t m, int32_t a_rows, int32_t n, int32_t k,
                    int32_t ldc, int32_t tile_n, int32_t split_k);
 
@@ -268,8 +277,9 @@ int lade_sample_verify_f16(LadeCtx* ctx, void* stream, const void* logits, int32
 
 /* ---- token selection / accept / pool update ---------------------------------------------------- */
 
-/* Row-wise argmax with lowest-index tie-break over bf16 logits [n_rows][vocab]
- * (torch.argmax at lade/decoding.py:1021,1041,1052,1072,1102). */
+/* Row-wise argmax with lowest-index tie-break over bf16 logits [n_rows][vocab], rows `ld` >= vocab elements apart
+ * (torch.argmax at lade/decoding.py:1021,1041,1052,1072,1102).  -inf and +inf compete like any value; a row of
+ * nothing but -inf gives 0.  NaN is outside the contract (torch.argmax would return its index; this does not). */
 int lade_argmax_rows(void* stream, const void* logits, int32_t n_rows, int32_t vocab, int32_t ld,
                      int32_t* out_idx);
 
@@ -347,8 +357,13 @@ int lade_sample_verify_warped_f16(LadeCtx* ctx, void* stream, const void* logits
 int lade_commit_decision(LadeCtx* ctx, void* stream, const int32_t* decision, const int32_t* meta,
                          int32_t* result);
 
-/* Move the accepted n-gram's K/V rows to the cache tail for every layer (lade/decoding.py:1156-1163).
- * k_base/v_base point at layer 0; layers are `layer_stride_elems` apart. */
+/* Move the accepted n-gram's K/V rows to the cache tail for every layer (lade/decoding.py:1156-1163): rows
+ * [R_KV_SRC, R_KV_SRC + h) of every head go to [R_KV_DST, R_KV_DST + h), h = min(R_MAX_HIT, max_rows); nothing moves when
+ * R_MAX_HIT is 0 or R_KV_SRC < 0.  k_base/v_base point at layer 0; layers are `layer_stride_elems` apart (at least
+ * n_kv_heads * kv_capacity * head_dim); 16-bit payloads of either model dtype.
+ * Precondition: the two row ranges do not overlap, R_KV_SRC - R_KV_DST >= R_MAX_HIT (every row is copied by its own
+ * CTA, in no order).  The results of lade_accept_update / lade_commit_decision satisfy it: the source rows are the
+ * step's guess rows, which lie behind all of its window rows, the destination the first rows after the input token. */
 int lade_kv_compact(void* stream, const int32_t* result, void* k_base, void* v_base,
                     int64_t layer_stride_elems, int32_t n_layers, int32_t n_kv_heads,
                     int32_t kv_capacity, int32_t head_dim, int32_t max_rows);

@@ -207,6 +207,10 @@ using namespace lade;
 
 extern "C" {
 
+// s_part of rmsnorm_kernel: it counts against the 48 KB a kernel may use without opting in, so a row of 12288 floats
+// (exactly 48 KB of dynamic shared memory) already needs the opt-in
+constexpr size_t NORM_STATIC_SMEM = 32 * sizeof(float);
+
 static int norm_threads(int hidden) {
   int t = ((hidden / 8 + 31) / 32) * 32;
   return t < 128 ? 128 : (t > 1024 ? 1024 : t);
@@ -221,7 +225,7 @@ static int rmsnorm_impl(void* stream, const void* x, const void* delta, const vo
   if (delta && !h_out) return LADE_EINVAL;
   const size_t smem = sizeof(float) * hidden;
   if (smem > 96 * 1024) return LADE_EUNSUPPORTED;
-  if (smem > 48 * 1024)
+  if (smem + NORM_STATIC_SMEM > 48 * 1024)
     LADE_CUDA_CHECK(cudaFuncSetAttribute(rmsnorm_kernel<false, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // one 16-byte vector per thread when the row fits (4096 / 8 = 512 threads): a single round of loads per phase
   const int threads = norm_threads(hidden);
@@ -237,7 +241,7 @@ static int rmsnorm_gather_impl(void* stream, const void* x, const void* delta, c
   if (!x || !weight || !out || !rows_idx || n_rows < 1 || hidden < 8 || hidden % 8 != 0) return LADE_EINVAL;
   const size_t smem = sizeof(float) * hidden;
   if (smem > 96 * 1024) return LADE_EUNSUPPORTED;
-  if (smem > 48 * 1024)
+  if (smem + NORM_STATIC_SMEM > 48 * 1024)
     LADE_CUDA_CHECK(cudaFuncSetAttribute(rmsnorm_kernel<true, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int threads = norm_threads(hidden);
   LADE_CUDA_CHECK(launch_pdl(rmsnorm_kernel<true, T>, dim3(n_rows), dim3(threads), smem, (cudaStream_t)stream,

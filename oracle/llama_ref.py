@@ -202,11 +202,99 @@ def bound_ratio(got: torch.Tensor, o_ref: torch.Tensor, bound: torch.Tensor) -> 
 MAX_RATIO, MEAN_RATIO = 1.0, 0.25
 
 
-def within_bound(got, o_ref, bound) -> Tuple[bool, float, float]:
-    """(passes, max ratio, mean ratio) of `got` against (o_ref, bound) of attention_fp64."""
+def within_bound(got, o_ref, bound, mean_ratio: float = MEAN_RATIO) -> Tuple[bool, float, float]:
+    """(passes, max ratio, mean ratio) of `got` against (o_ref, bound) of attention_fp64 or linear_fp64."""
     ratio = bound_ratio(got, o_ref, bound)
     mx, mean = ratio.max().item(), ratio.mean().item()
-    return mx <= MAX_RATIO and mean <= MEAN_RATIO, mx, mean
+    return mx <= MAX_RATIO and mean <= mean_ratio, mx, mean
+
+
+# ---- float64 projection GEMM and its error bound ------------------------------------------------------------------
+# A correctly rounded output alone has a mean error of a quarter ulp, 0.5 of the bound's half-ulp term, so the mean
+# criterion of a GEMM output is 0.55: where the accumulation term is small an honest kernel sits at 0.5, lower
+# elsewhere; an output rounded any other way than to nearest does not.
+LINEAR_MEAN_RATIO = 0.55
+
+
+def linear_gamma(K: int) -> float:
+    """Relative weight of sum_k |a_k w_k| in the bound of linear_fp64 (derivation there)."""
+    return (K / 16 + 4 + 8) * 2.0 ** -23
+
+
+def linear_fp64(a: torch.Tensor, w: torch.Tensor, dtype) -> Tuple[torch.Tensor, torch.Tensor]:
+    """nn.Linear without bias in float64, c = a . w^T for a [M, K], w [N, K] (model dtype values), and a per-element
+    bound on how far a kernel that accumulates in fp32 and rounds once to `dtype` may be from it.
+
+    Returns (ref, bound), float64 [M, N]:
+        bound = ulp_T(ref) / 2 + gamma * (|a| . |w|^T),    gamma = (K / 16 + 4 + 8) * 2^-23.
+    * ulp_T(ref) / 2: the single rounding of the fp32 result to the model dtype.  (A result that the accumulation error
+      d pushes over a power of two rounds with the coarser spacing, but the power of two itself is representable, so
+      the rounding moves it by at most d more; the slack of gamma covers that.)
+    * gamma: the products of two model-dtype values are exact in fp32.  Every k16 step of the tensor core adds one
+      16-term sum to the accumulator: K / 16 sequential fp32 additions; the 16-term sum counts as a 4-level tree; up to
+      8 split-K partials add at most 8 more.  Each addition is charged 2^-23, not the 2^-24 of round-to-nearest,
+      because the tensor core may truncate where IEEE would round.  All of them act on partial sums of magnitude at
+      most sum_k |a_k w_k|.
+    Integer operands whose partial sums stay below 2^24 make every addition exact whatever the order: then a kernel
+    must return T(ref) bit for bit, which the exact probes of the tests use."""
+    ad, wd = a.double(), w.double()
+    ref = ad @ wd.t()
+    bound = 0.5 * ulp(ref, dtype) + linear_gamma(a.shape[-1]) * (ad.abs() @ wd.abs().t())
+    return ref, bound
+
+
+# ---- float64 RMSNorm and SwiGLU with the kernels' rounding points -------------------------------------------------
+# Both return the result and, per element, the other admissible result: where the value that is rounded to the model
+# dtype lies so close to a rounding midpoint that the fp32 arithmetic in front of it may tip it either way, the
+# neighbouring model-dtype number is as correct as the nearest one.  A kernel output is right iff it equals the first
+# tensor, or the second where the two differ; `unexplained` counts the rest.
+NORM_WINDOW_ULPS, SILU_WINDOW_ULPS = 8, 8
+
+
+def rms_norm_fp64(x, delta, w, eps: float, dtype):
+    """LlamaRMSNorm with the fused residual add (modeling_llama.py:222-227, :883-889), T = `dtype`:
+        h = T(x + delta)  (torch's model-dtype add; delta may be None), n = T(h * rstd), out = T(w * n),
+        rstd = 1 / sqrt(mean(h^2) + fp32(eps)) in float64.
+    Returns (h, out, out_alt).  n has an alternative where h * rstd is within a relative (hidden + 8) * 2^-24 of a
+    rounding midpoint: the fp32 sum of `hidden` squares in any order is off by at most hidden * 2^-24 relative, and
+    the division, the addition of eps, rsqrtf (2 ulp) and the final product add less than 8 * 2^-24.  w * n is the
+    product of two model-dtype numbers, exact in fp32, so the last rounding has no alternative of its own."""
+    h = x if delta is None else x + delta
+    hd = h.double()
+    hidden = h.shape[-1]
+    eps32 = float(torch.tensor(eps, dtype=torch.float32))
+    rstd = 1.0 / torch.sqrt(hd.pow(2).mean(-1, keepdim=True) + eps32)
+    v = hd * rstd
+    n, n_alt = _round_alternative(v, dtype, (hidden + NORM_WINDOW_ULPS) * 2.0 ** -24 * v.abs())
+    wd = w.double()
+    return h, (wd * n).to(dtype), (wd * n_alt).to(dtype)
+
+
+_LOG_FLT_MAX = math.log(float(torch.finfo(torch.float32).max))
+
+
+def swiglu_fp64(gate_up: torch.Tensor, dtype):
+    """LlamaMLP's act_fn(gate) * up (modeling_llama.py:378) on the fused [rows, 2 * inter] projection, T = `dtype`:
+        s = T(silu(g)), out = T(s * u),   silu(g) = g / (1 + exp(-g)) in float64.
+    Returns (out, out_alt).  s has an alternative where silu(g) is within a relative 8 * 2^-24 of a rounding midpoint
+    (expf 2 ulp, the addition, the division, with room to spare).  The reference evaluates silu in fp32, where exp(-g)
+    overflows for g < -88.72 and the quotient is -0; the restatement says -0 there too (bf16 could represent the
+    float64 value, about -1e-37).  s * u is exact in fp32; an fp16 product beyond 65504 is inf in both."""
+    inter = gate_up.shape[-1] // 2
+    g, u = gate_up[..., :inter].double(), gate_up[..., inter:].double()
+    v = g / (1.0 + torch.exp(-g))
+    v = torch.where(-g > _LOG_FLT_MAX, -torch.zeros_like(g), v)
+    s, s_alt = _round_alternative(v, dtype, SILU_WINDOW_ULPS * 2.0 ** -24 * v.abs())
+    return (s * u).to(dtype), (s_alt * u).to(dtype)
+
+
+def unexplained(got: torch.Tensor, main: torch.Tensor, alt: torch.Tensor) -> Tuple[int, int]:
+    """(elements of `got` that equal neither `main` nor `alt`, elements that needed `alt`); NaN equals only NaN."""
+    def same(p, q):
+        return (p == q) | (torch.isnan(p) & torch.isnan(q))
+    is_main = same(got, main)
+    is_alt = same(got, alt)
+    return int((~is_main & ~is_alt).sum()), int((~is_main & is_alt).sum())
 
 
 class OracleLlama:
