@@ -245,6 +245,39 @@ int lade_debug_attn_pdl(int32_t enable);
 int lade_gemm_bf16(void* stream, const void* a, const void* w, void* c, int32_t m, int32_t a_rows, int32_t n, int32_t k,
                    int32_t ldc, int32_t tile_n, int32_t split_k);
 
+/* FP8 projection, T = bf16 (lade_gemm_fp8) or fp16 (lade_gemm_fp8_f16); not on the engine's step (DESIGN.md §7.2):
+ *   c[r][n] = T( __fmul_rn(__fmul_rn(sum_k a[r][k] * w[n][k], a_scale[r]), w_scale[n]) )
+ * a: [a_rows][k] and w: [n][k] float8_e4m3fn bytes, row-major (the nn.Linear layout, K-major for wgmma); a_scale: [m]
+ * and w_scale: [n] fp32, the scales of the row quantisation of lade_quant_rows_fp8 (see there).  The sum runs over
+ * 128-deep k-blocks: each block on the tensor cores (m64nNk32 e4m3 wgmma into a zeroed accumulator), then added in fp32
+ * on the CUDA cores; K splits are added in split order before the scales.  Requires k % 128 == 0, n % 8 == 0,
+ * ldc % 8 == 0, ldc >= n, 16-byte aligned a / w / c.  Up to 256 rows stream each weight once; larger m loops over
+ * 256-row chunks.  tile_n (32..128, multiple of 32; bits 16-19 a ring-depth cap, bit 20 = no ring prefill before the
+ * CTA barrier) and split_k as for lade_gemm_bf16; the automatic choice depends on (n, k) only, so an output row is
+ * the same bits whatever m is.  A rejected configuration returns LADE_EINVAL before anything is written. */
+int lade_gemm_fp8(void* stream, const void* a, const float* a_scale, const void* w, const float* w_scale, void* c,
+                  int32_t m, int32_t a_rows, int32_t n, int32_t k, int32_t ldc, int32_t tile_n, int32_t split_k);
+int lade_gemm_fp8_f16(void* stream, const void* a, const float* a_scale, const void* w, const float* w_scale, void* c,
+                      int32_t m, int32_t a_rows, int32_t n, int32_t k, int32_t ldc, int32_t tile_n, int32_t split_k);
+
+/* e4m3 row quantisation, the same for activations (per token) and weights (per output channel).  For a row x of T:
+ *   amax = max |x| (fp32); s = amax / 448 (fp32), or 1 when amax is 0 or not finite; q = e4m3(x / s) with the division
+ *   in fp32, round to nearest even, saturated to +-448 (float8_e4m3fn).  A row holding inf or NaN quantises to
+ *   undefined bytes.
+ * lade_rmsnorm_quant_fp8: lade_rmsnorm's output row T(w * n), quantised to q_out [rows][hidden] / s_out [rows] instead
+ *   of stored (h_out as in lade_rmsnorm).
+ * lade_swiglu_quant_fp8: lade_swiglu's row T(T(silu(g)) * u), quantised to q_out [rows][inter] / s_out [rows].
+ * lade_quant_rows_fp8: plain rows x [rows][cols] to q_out [rows][cols] / s_out [rows].
+ * Every output row depends only on its own input row.  _f16: the fp16 twins. */
+int lade_rmsnorm_quant_fp8(void* stream, const void* x, const void* delta, const void* weight, void* h_out, void* q_out,
+                           float* s_out, int32_t rows, int32_t hidden, float eps);
+int lade_rmsnorm_quant_fp8_f16(void* stream, const void* x, const void* delta, const void* weight, void* h_out, void* q_out,
+                               float* s_out, int32_t rows, int32_t hidden, float eps);
+int lade_swiglu_quant_fp8(void* stream, const void* gate_up, void* q_out, float* s_out, int32_t rows, int32_t inter);
+int lade_swiglu_quant_fp8_f16(void* stream, const void* gate_up, void* q_out, float* s_out, int32_t rows, int32_t inter);
+int lade_quant_rows_fp8(void* stream, const void* x, void* q_out, float* s_out, int32_t rows, int32_t cols);
+int lade_quant_rows_fp8_f16(void* stream, const void* x, void* q_out, float* s_out, int32_t rows, int32_t cols);
+
 /* Profiling aid: when set (device buffer of 4 * 1024 * 8 int64, or NULL to disable) the GEMM kernel records
  * %globaltimer (ns) at its phase boundaries per CTA, the last 4 launches round-robin. */
 int lade_debug_gemm_timing(void* dev_buffer);

@@ -65,6 +65,10 @@ _SIGNATURES = {
     "lade_debug_attn_timing": (C.c_int, [c_p]),
     "lade_debug_attn_pdl": (C.c_int, [c_i32]),
     "lade_gemm_bf16": (C.c_int, [c_p, c_p, c_p, c_p, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
+    "lade_gemm_fp8": (C.c_int, [c_p, c_p, c_p, c_p, c_p, c_p] + [c_i32] * 7),
+    "lade_rmsnorm_quant_fp8": (C.c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i32, c_i32, C.c_float]),
+    "lade_swiglu_quant_fp8": (C.c_int, [c_p, c_p, c_p, c_p, c_i32, c_i32]),
+    "lade_quant_rows_fp8": (C.c_int, [c_p, c_p, c_p, c_p, c_i32, c_i32]),
     "lade_debug_gemm_timing": (C.c_int, [c_p]),
     "lade_swiglu": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32]),
     "lade_argmax_rows": (C.c_int, [c_p, c_p, c_i32, c_i32, c_i32, c_p]),
@@ -94,7 +98,8 @@ _SIGNATURES = {
 
 # fp16 twins: same signatures as the bf16 entry points
 for _name in ("lade_rmsnorm", "lade_rmsnorm_gather", "lade_rope_append", "lade_swiglu", "lade_argmax_rows", "lade_attn_fwd",
-              "lade_sample_verify", "lade_argmax_processed", "lade_sample_verify_warped"):
+              "lade_sample_verify", "lade_argmax_processed", "lade_sample_verify_warped", "lade_gemm_fp8",
+              "lade_rmsnorm_quant_fp8", "lade_swiglu_quant_fp8", "lade_quant_rows_fp8"):
     _SIGNATURES[_name + "_f16"] = _SIGNATURES[_name]
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

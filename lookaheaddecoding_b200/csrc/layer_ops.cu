@@ -3,7 +3,15 @@
 //   rotary embedding + KV append     lade/models/modeling_llama.py:342-346, :513-516
 //   SwiGLU                            lade/models/modeling_llama.py:378
 // All are HBM-bound byte movers: 16-byte vectorised, coalesced, one pass over the data.
+//
+// The FP8 projections (lade_gemm_fp8) take their activations from variants of the RMSNorm and SwiGLU kernels that
+// quantise the row they produce instead of storing it, and from lade_quant_rows_fp8 (attention output, weights).  Row quantisation, the same for activations (per token) and weights (per output channel):
+//   amax = max |x| over the row (fp32, of the row rounded to the model dtype T),
+//   s = amax / 448 in fp32, or 1 when amax is 0 or not finite (a row holding inf / NaN quantises to garbage),
+//   q = e4m3(x / s): fp32 division, round to nearest even, saturated to +-448 (float8_e4m3fn).
 #include "common.cuh"
+
+#include <cuda_fp8.h>
 
 #include <cstdlib>
 
@@ -49,14 +57,69 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// ---- e4m3 row quantisation --------------------------------------------------------------------------------
+// max over the CTA (fmaxf: a NaN element is skipped); `s_part` (32 floats) must not be in use by another phase
+__device__ __forceinline__ float block_max(float v, float* s_part) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float m = 0.f;
+  for (int k = 0; k < (int)(blockDim.x >> 5); ++k) m = fmaxf(m, s_part[k]);
+  return m;
+}
+__device__ __forceinline__ float fp8_row_scale(float amax) {
+  return (amax > 0.f && amax <= 3.402823466e38f) ? __fdiv_rn(amax, 448.f) : 1.f;
+}
+// 8 values -> 8 e4m3 bytes (element j in byte j)
+__device__ __forceinline__ uint2 fp8_pack8(const float (&f)[8], float s) {
+  uint32_t w[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    uint32_t b = 0;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const float2 v = make_float2(__fdiv_rn(f[4 * h + 2 * j], s), __fdiv_rn(f[4 * h + 2 * j + 1], s));
+      b |= (uint32_t)__nv_cvt_float2_to_fp8x2(v, __NV_SATFINITE, __NV_E4M3) << (16 * j);
+    }
+    w[h] = b;
+  }
+  return make_uint2(w[0], w[1]);
+}
+// One CTA quantises one row of `nvec` 8-element vectors produced by vec(c) (a uint4 of 8 T values): a pass for the
+// amax, a second one (vec is recomputed) for the bytes.
+template <typename T, typename F>
+__device__ __forceinline__ void quant_row(F vec, int nvec, uint8_t* __restrict__ q_row, float* __restrict__ s_slot,
+                                          float* s_part) {
+  float amax = 0.f;
+  for (int c = threadIdx.x; c < nvec; c += blockDim.x) {
+    const uint4 v = vec(c);
+    const T* e = reinterpret_cast<const T*>(&v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(Elem<T>::to_f(e[j])));
+  }
+  const float s = fp8_row_scale(block_max(amax, s_part));
+  for (int c = threadIdx.x; c < nvec; c += blockDim.x) {
+    const uint4 v = vec(c);
+    const T* e = reinterpret_cast<const T*>(&v);
+    float f[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f[j] = Elem<T>::to_f(e[j]);
+    reinterpret_cast<uint2*>(q_row)[c] = fp8_pack8(f, s);
+  }
+  if (threadIdx.x == 0) *s_slot = s;
+}
+
 // One CTA per row.  h = bf16(x + delta) (if delta), out = w * bf16(h_f32 * rsqrt(mean(h^2) + eps)).
-template <bool GATHER, typename T>
+// QUANT: the output row is not stored but quantised to e4m3 (q_out, s_out) instead.
+template <bool GATHER, typename T, bool QUANT = false>
 __global__ void __launch_bounds__(1024) rmsnorm_kernel(const T* __restrict__ x,
                                                       const T* __restrict__ delta,
                                                       const T* __restrict__ w,
                                                       const int* __restrict__ rows_idx,
                                                       T* __restrict__ h_out,
-                                                      T* __restrict__ out, int hidden, float eps) {
+                                                      T* __restrict__ out, int hidden, float eps,
+                                                      uint8_t* __restrict__ q_out, float* __restrict__ s_out) {
   extern __shared__ float s_row[];  // hidden floats
   __shared__ float s_part[32];
   pdl_enter();
@@ -96,6 +159,7 @@ __global__ void __launch_bounds__(1024) rmsnorm_kernel(const T* __restrict__ x,
   for (int k = 0; k < (int)(blockDim.x >> 5); ++k) tot += s_part[k];
   const float rstd = rsqrtf(tot / (float)hidden + eps);
   T* orow = out + (long long)out_row * hidden;
+  float amax = 0.f;
   for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
     uint4 wv = reinterpret_cast<const uint4*>(w)[i];
     const T* we = reinterpret_cast<const T*>(&wv);
@@ -106,7 +170,27 @@ __global__ void __launch_bounds__(1024) rmsnorm_kernel(const T* __restrict__ x,
       const float n = round_to<T>(s_row[i * 8 + j] * rstd);                // .to(input_dtype)
       oe[j] = Elem<T>::from_f(Elem<T>::to_f(we[j]) * n);                   // weight * hidden (model-dtype mul)
     }
-    reinterpret_cast<uint4*>(orow)[i] = ov;
+    if constexpr (QUANT) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {                                        // this thread's slots of s_row only
+        s_row[i * 8 + j] = Elem<T>::to_f(oe[j]);
+        amax = fmaxf(amax, fabsf(s_row[i * 8 + j]));
+      }
+    } else {
+      reinterpret_cast<uint4*>(orow)[i] = ov;
+    }
+  }
+  if constexpr (QUANT) {
+    __syncthreads();                                                       // every thread has read s_part above
+    const float s = fp8_row_scale(block_max(amax, s_part));
+    uint8_t* qrow = q_out + (long long)out_row * hidden;
+    for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+      float f[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = s_row[i * 8 + j];
+      reinterpret_cast<uint2*>(qrow)[i] = fp8_pack8(f, s);
+    }
+    if (threadIdx.x == 0) s_out[out_row] = s;
   }
 }
 
@@ -176,6 +260,24 @@ __global__ void __launch_bounds__(1024) rope_append_kernel(
   }
 }
 
+// 8 elements of row r of the fused [rows][2*inter] gate/up projection: T(T(silu(g)) * u)
+template <typename T>
+__device__ __forceinline__ uint4 swiglu8(const T* __restrict__ gate_up, int r, int c, int inter) {
+  const uint4 gv = reinterpret_cast<const uint4*>(gate_up + (long long)r * 2 * inter)[c];
+  const uint4 uv = reinterpret_cast<const uint4*>(gate_up + (long long)r * 2 * inter + inter)[c];
+  const T* g = reinterpret_cast<const T*>(&gv);
+  const T* u = reinterpret_cast<const T*>(&uv);
+  uint4 ov;
+  T* o = reinterpret_cast<T*>(&ov);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float x = Elem<T>::to_f(g[j]);
+    const float s = round_to<T>(x / (1.0f + expf(-x)));                     // silu in fp32, model-dtype result
+    o[j] = Elem<T>::from_f(s * Elem<T>::to_f(u[j]));
+  }
+  return ov;
+}
+
 template <typename T>
 __global__ void swiglu_kernel(const T* __restrict__ gate_up, T* __restrict__ out,
                               int rows, int inter) {
@@ -185,20 +287,29 @@ __global__ void swiglu_kernel(const T* __restrict__ gate_up, T* __restrict__ out
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const int r = (int)(i / nvec), c = (int)(i % nvec);
-    const uint4 gv = reinterpret_cast<const uint4*>(gate_up + (long long)r * 2 * inter)[c];
-    const uint4 uv = reinterpret_cast<const uint4*>(gate_up + (long long)r * 2 * inter + inter)[c];
-    const T* g = reinterpret_cast<const T*>(&gv);
-    const T* u = reinterpret_cast<const T*>(&uv);
-    uint4 ov;
-    T* o = reinterpret_cast<T*>(&ov);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float x = Elem<T>::to_f(g[j]);
-      const float s = round_to<T>(x / (1.0f + expf(-x)));                   // silu in fp32, model-dtype result
-      o[j] = Elem<T>::from_f(s * Elem<T>::to_f(u[j]));
-    }
-    reinterpret_cast<uint4*>(out + (long long)r * inter)[c] = ov;
+    reinterpret_cast<uint4*>(out + (long long)r * inter)[c] = swiglu8(gate_up, r, c, inter);
   }
+}
+
+// SwiGLU quantised to e4m3: one CTA per row (the scale needs the row's amax)
+template <typename T>
+__global__ void __launch_bounds__(1024) swiglu_quant_kernel(const T* __restrict__ gate_up, uint8_t* __restrict__ q_out,
+                                                            float* __restrict__ s_out, int inter) {
+  __shared__ float s_part[32];
+  pdl_enter();
+  const int r = blockIdx.x;
+  quant_row<T>([&](int c) { return swiglu8(gate_up, r, c, inter); }, inter / 8, q_out + (long long)r * inter, s_out + r, s_part);
+}
+
+// Plain rows quantised to e4m3 (the attention output before o_proj; the weights, once, per output channel)
+template <typename T>
+__global__ void __launch_bounds__(1024) quant_rows_kernel(const T* __restrict__ x, uint8_t* __restrict__ q_out,
+                                                          float* __restrict__ s_out, int cols) {
+  __shared__ float s_part[32];
+  pdl_enter();
+  const int r = blockIdx.x;
+  const uint4* xr = reinterpret_cast<const uint4*>(x + (long long)r * cols);
+  quant_row<T>([&](int c) { return xr[c]; }, cols / 8, q_out + (long long)r * cols, s_out + r, s_part);
 }
 
 }  // namespace lade
@@ -231,7 +342,23 @@ static int rmsnorm_impl(void* stream, const void* x, const void* delta, const vo
   const int threads = norm_threads(hidden);
   LADE_CUDA_CHECK(launch_pdl(rmsnorm_kernel<false, T>, dim3(rows), dim3(threads), smem, (cudaStream_t)stream,
                              (const T*)x, (const T*)delta, (const T*)weight, (const int*)nullptr, (T*)h_out, (T*)out,
-                             hidden, eps));
+                             hidden, eps, (uint8_t*)nullptr, (float*)nullptr));
+  return LADE_OK;
+}
+
+template <typename T>
+static int rmsnorm_quant_impl(void* stream, const void* x, const void* delta, const void* weight, void* h_out, void* q_out,
+                              float* s_out, int32_t rows, int32_t hidden, float eps) {
+  if (!x || !weight || !q_out || !s_out || rows < 1 || hidden < 8 || hidden % 8 != 0) return LADE_EINVAL;
+  if (delta && !h_out) return LADE_EINVAL;
+  const size_t smem = sizeof(float) * hidden;
+  if (smem > 96 * 1024) return LADE_EUNSUPPORTED;
+  if (smem + NORM_STATIC_SMEM > 48 * 1024)
+    LADE_CUDA_CHECK(cudaFuncSetAttribute(rmsnorm_kernel<false, T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int threads = norm_threads(hidden);
+  LADE_CUDA_CHECK(launch_pdl(rmsnorm_kernel<false, T, true>, dim3(rows), dim3(threads), smem, (cudaStream_t)stream,
+                             (const T*)x, (const T*)delta, (const T*)weight, (const int*)nullptr, (T*)h_out, (T*)nullptr,
+                             hidden, eps, (uint8_t*)q_out, s_out));
   return LADE_OK;
 }
 
@@ -246,7 +373,7 @@ static int rmsnorm_gather_impl(void* stream, const void* x, const void* delta, c
   const int threads = norm_threads(hidden);
   LADE_CUDA_CHECK(launch_pdl(rmsnorm_kernel<true, T>, dim3(n_rows), dim3(threads), smem, (cudaStream_t)stream,
                              (const T*)x, (const T*)delta, (const T*)weight, (const int*)rows_idx, (T*)nullptr, (T*)out,
-                             hidden, eps));
+                             hidden, eps, (uint8_t*)nullptr, (float*)nullptr));
   return LADE_OK;
 }
 
@@ -274,6 +401,22 @@ static int swiglu_impl(void* stream, const void* gate_up, void* out, int32_t row
   if (blocks > 132 * 8) blocks = 132 * 8;
   LADE_CUDA_CHECK(launch_pdl(swiglu_kernel<T>, dim3(blocks), dim3(256), 0, (cudaStream_t)stream,
                              (const T*)gate_up, (T*)out, rows, inter));
+  return LADE_OK;
+}
+
+template <typename T>
+static int swiglu_quant_impl(void* stream, const void* gate_up, void* q_out, float* s_out, int32_t rows, int32_t inter) {
+  if (!gate_up || !q_out || !s_out || rows < 1 || inter < 8 || inter % 8 != 0) return LADE_EINVAL;
+  LADE_CUDA_CHECK(launch_pdl(swiglu_quant_kernel<T>, dim3(rows), dim3(norm_threads(inter)), 0, (cudaStream_t)stream,
+                             (const T*)gate_up, (uint8_t*)q_out, s_out, inter));
+  return LADE_OK;
+}
+
+template <typename T>
+static int quant_rows_impl(void* stream, const void* x, void* q_out, float* s_out, int32_t rows, int32_t cols) {
+  if (!x || !q_out || !s_out || rows < 1 || cols < 8 || cols % 8 != 0) return LADE_EINVAL;
+  LADE_CUDA_CHECK(launch_pdl(quant_rows_kernel<T>, dim3(rows), dim3(norm_threads(cols)), 0, (cudaStream_t)stream,
+                             (const T*)x, (uint8_t*)q_out, s_out, cols));
   return LADE_OK;
 }
 
@@ -316,6 +459,26 @@ int lade_swiglu(void* stream, const void* gate_up, void* out, int32_t rows, int3
 }
 int lade_swiglu_f16(void* stream, const void* gate_up, void* out, int32_t rows, int32_t inter) {
   return swiglu_impl<__half>(stream, gate_up, out, rows, inter);
+}
+int lade_rmsnorm_quant_fp8(void* stream, const void* x, const void* delta, const void* weight, void* h_out, void* q_out,
+                           float* s_out, int32_t rows, int32_t hidden, float eps) {
+  return rmsnorm_quant_impl<__nv_bfloat16>(stream, x, delta, weight, h_out, q_out, s_out, rows, hidden, eps);
+}
+int lade_rmsnorm_quant_fp8_f16(void* stream, const void* x, const void* delta, const void* weight, void* h_out, void* q_out,
+                               float* s_out, int32_t rows, int32_t hidden, float eps) {
+  return rmsnorm_quant_impl<__half>(stream, x, delta, weight, h_out, q_out, s_out, rows, hidden, eps);
+}
+int lade_swiglu_quant_fp8(void* stream, const void* gate_up, void* q_out, float* s_out, int32_t rows, int32_t inter) {
+  return swiglu_quant_impl<__nv_bfloat16>(stream, gate_up, q_out, s_out, rows, inter);
+}
+int lade_swiglu_quant_fp8_f16(void* stream, const void* gate_up, void* q_out, float* s_out, int32_t rows, int32_t inter) {
+  return swiglu_quant_impl<__half>(stream, gate_up, q_out, s_out, rows, inter);
+}
+int lade_quant_rows_fp8(void* stream, const void* x, void* q_out, float* s_out, int32_t rows, int32_t cols) {
+  return quant_rows_impl<__nv_bfloat16>(stream, x, q_out, s_out, rows, cols);
+}
+int lade_quant_rows_fp8_f16(void* stream, const void* x, void* q_out, float* s_out, int32_t rows, int32_t cols) {
+  return quant_rows_impl<__half>(stream, x, q_out, s_out, rows, cols);
 }
 
 }  // extern "C"

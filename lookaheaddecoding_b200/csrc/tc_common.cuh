@@ -110,6 +110,14 @@ __device__ __forceinline__ void wgmma_m64n32_ss_bf16(float (&d)[16], uint64_t da
                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, 1, 1, 1, 0, 0;"
                : LADE_WG_O16(d, 0) : "l"(da), "l"(db));
 }
+// D[64 x 32] (+)= A[64 x 32] . B[32 x 32], e4m3, both K-major from shared memory (the only layout fp8 wgmma has);
+// accumulate == 0 zeroes D first.
+__device__ __forceinline__ void wgmma_m64n32k32_ss_e4m3(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 "
+               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+               : LADE_WG_O16(d, 0) : "l"(da), "l"(db), "r"(accumulate));
+}
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
