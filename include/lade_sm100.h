@@ -191,6 +191,27 @@ int lade_rope_append(void* stream, const void* qkv, const void* cos_tab, const v
                      int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
                      int32_t kv_capacity, int32_t max_pos);
 
+/* Qwen3 variant (Qwen3ForCausalLM): the per-head RMSNorm of q and of k in front of the rotary embedding, fused into the
+ * same pass.  Qwen3Attention.forward (transformers modeling_qwen3.py):
+ *     query_states = self.q_norm(self.q_proj(hidden_states).view(hidden_shape))      (the same for k with k_norm)
+ *     query_states, key_states = apply_rotary_pos_emb(query_states, key_states, cos, sin)
+ * with Qwen3RMSNorm.forward, the rounding points of LlamaRMSNorm, over each head of D elements:
+ *     rstd = rsqrt(sum(x^2) / D + eps)  (fp32),  n = T(x * rstd),  y = T(w * n)
+ * then the rotary embedding of lade_rope_append on y, with its roundings.  V is appended unchanged.
+ * q_norm_w, k_norm_w: device T[head_dim] (the two modules' weights), 16-byte aligned; eps: the modules'
+ * variance_epsilon.  Arguments, layouts and errors otherwise as lade_rope_append; LADE_EINVAL also for a null or
+ * misaligned weight, eps negative or not finite, and head_dim / 16 not a power of two.  Nothing is launched on an
+ * error.  _f16: fp16 models. */
+int lade_rope_append_qknorm(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab,
+                            const int32_t* pos, const int32_t* meta, void* q_out, void* k_cache, void* v_cache,
+                            int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
+                            int32_t kv_capacity, int32_t max_pos, const void* q_norm_w, const void* k_norm_w, float eps);
+int lade_rope_append_qknorm_f16(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab,
+                                const int32_t* pos, const int32_t* meta, void* q_out, void* k_cache, void* v_cache,
+                                int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
+                                int32_t kv_capacity, int32_t max_pos, const void* q_norm_w, const void* k_norm_w,
+                                float eps);
+
 /* Lookahead attention over the persistent KV cache (the roofline kernel).  softmax(QK^T/sqrt(D) +
  * lookahead mask) V with the mask bits of `rowmask` tested in registers (prefill steps: plain causal,
  * rowmask unused); all step rows see the committed cache.  Replaces LlamaAttention.forward's attention core (modeling_llama.py:520-541), the

@@ -1,6 +1,7 @@
 // Memory-bound glue kernels of the decoder layer, with the reference's bf16 rounding points.
 //   RMSNorm (+ fused residual add)   lade/models/modeling_llama.py:222-227, :883-889
 //   rotary embedding + KV append     lade/models/modeling_llama.py:342-346, :513-516
+//   (Qwen3: per-head q/k RMSNorm in front of the rotary embedding, fused into the same kernel)
 //   SwiGLU                            lade/models/modeling_llama.py:378
 // All are HBM-bound byte movers: 16-byte vectorised, coalesced, one pass over the data.
 //
@@ -197,12 +198,20 @@ __global__ void __launch_bounds__(1024) rmsnorm_kernel(const T* __restrict__ x,
 // RoPE + append.  grid: rows ; block: 256 threads.  Work item = (head, 8-wide slice of the first half):
 // the thread rotates elements [8i, 8i+8) of the first half against the same slice of the second half,
 // all accesses 16 bytes.  (Hq + 2 Hkv) * D/16 items per row.
-template <typename T>
+// QKNORM (Qwen3Attention.forward: q_norm / k_norm over each head, then apply_rotary_pos_emb): every q and k head is
+// first replaced by T(w * T(x * rstd)), rstd = rsqrt(sum(x^2) / D + eps) in fp32, with w = q_norm_w or k_norm_w
+// ([D], the model dtype).  The D/16 items of a head are D/16 consecutive lanes of one warp in the same loop round
+// (D/16 divides 32 and blockDim.x is a multiple of 32; the host admits no other head_dim), so the head's sum of
+// squares is a shuffle reduction inside that lane group.  A group enters or leaves the loop, the V branch and the
+// capacity test as a whole (n_items is a multiple of D/16; the other two depend on the head and the row only), so
+// every lane of the group's shuffle mask reaches the shuffle.
+template <typename T, bool QKNORM>
 __global__ void __launch_bounds__(1024) rope_append_kernel(
     const T* __restrict__ qkv, const T* __restrict__ cos_tab,
     const T* __restrict__ sin_tab, const int* __restrict__ pos, const int* __restrict__ meta,
     T* __restrict__ q_out, T* __restrict__ k_cache, T* __restrict__ v_cache,
-    int q_pad, int n_heads, int n_kv_heads, int D, int kv_capacity, int max_pos) {
+    int q_pad, int n_heads, int n_kv_heads, int D, int kv_capacity, int max_pos,
+    const T* __restrict__ q_norm_w, const T* __restrict__ k_norm_w, float eps) {
   // programmatic dependent launch: let the consumer (lade_attn_fwd) start its prologue and prefetch the cache tiles of
   // earlier steps while this grid runs; it orders itself with griddepcontrol.wait before touching what is written here
   pdl_enter();
@@ -220,8 +229,8 @@ __global__ void __launch_bounds__(1024) rope_append_kernel(
   for (int it = threadIdx.x; it < n_items; it += blockDim.x) {
     const int h = it / per_head, sl = it % per_head;
     const T* src = qkv + (long long)r * ld + (long long)h * D + sl * 8;
-    const uint4 a = *reinterpret_cast<const uint4*>(src);
-    const uint4 b = *reinterpret_cast<const uint4*>(src + half);
+    uint4 a = *reinterpret_cast<const uint4*>(src);
+    uint4 b = *reinterpret_cast<const uint4*>(src + half);
     T* dst;
     if (h < n_heads) {
       dst = q_out + ((long long)h * q_pad + r) * D + sl * 8;
@@ -234,6 +243,30 @@ __global__ void __launch_bounds__(1024) rope_append_kernel(
       *reinterpret_cast<uint4*>(dst) = a;
       *reinterpret_cast<uint4*>(dst + half) = b;
       continue;
+    }
+    if constexpr (QKNORM) {
+      T* x1 = reinterpret_cast<T*>(&a);
+      T* x2 = reinterpret_cast<T*>(&b);
+      float ss = 0.f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float f1 = Elem<T>::to_f(x1[j]), f2 = Elem<T>::to_f(x2[j]);
+        ss += f1 * f1 + f2 * f2;
+      }
+      const int lane = threadIdx.x & 31;
+      const unsigned group = per_head == 32 ? 0xffffffffu : ((1u << per_head) - 1u) << (lane & ~(per_head - 1));
+      for (int o = per_head >> 1; o > 0; o >>= 1) ss += __shfl_xor_sync(group, ss, o);
+      const float rstd = rsqrtf(ss / (float)D + eps);
+      const T* w = h < n_heads ? q_norm_w : k_norm_w;
+      const uint4 w1v = *reinterpret_cast<const uint4*>(w + sl * 8);
+      const uint4 w2v = *reinterpret_cast<const uint4*>(w + half + sl * 8);
+      const T* w1 = reinterpret_cast<const T*>(&w1v);
+      const T* w2 = reinterpret_cast<const T*>(&w2v);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {                      // .to(input_dtype), then weight * hidden in the model dtype
+        x1[j] = Elem<T>::from_f(Elem<T>::to_f(w1[j]) * round_to<T>(Elem<T>::to_f(x1[j]) * rstd));
+        x2[j] = Elem<T>::from_f(Elem<T>::to_f(w2[j]) * round_to<T>(Elem<T>::to_f(x2[j]) * rstd));
+      }
     }
     const uint4 c1 = *reinterpret_cast<const uint4*>(crow + sl * 8);
     const uint4 c2 = *reinterpret_cast<const uint4*>(crow + half + sl * 8);
@@ -377,19 +410,25 @@ static int rmsnorm_gather_impl(void* stream, const void* x, const void* delta, c
   return LADE_OK;
 }
 
-template <typename T>
+template <typename T, bool QKNORM = false>
 static int rope_append_impl(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab, const int32_t* pos,
                             const int32_t* meta, void* q_out, void* k_cache, void* v_cache, int32_t rows, int32_t q_pad,
-                            int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, int32_t kv_capacity, int32_t max_pos) {
+                            int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, int32_t kv_capacity, int32_t max_pos,
+                            const void* q_norm_w = nullptr, const void* k_norm_w = nullptr, float eps = 0.f) {
   if (!qkv || !cos_tab || !sin_tab || !pos || !meta || !q_out || !k_cache || !v_cache) return LADE_EINVAL;
   if (rows < 1 || rows > q_pad || head_dim % 16 != 0 || head_dim > 512 || n_heads < 1 || n_kv_heads < 1) return LADE_EINVAL;
+  if (QKNORM) {
+    // a head's D/16 lanes must be an aligned group inside one warp: D/16 a power of two (D in {16, 32, ..., 512})
+    if (!q_norm_w || !k_norm_w || ((uintptr_t)q_norm_w & 15) || ((uintptr_t)k_norm_w & 15)) return LADE_EINVAL;
+    if (((head_dim / 16) & (head_dim / 16 - 1)) != 0 || !(eps >= 0.f && eps <= 3.402823466e38f)) return LADE_EINVAL;
+  }
   // one work item (head, 8-wide slice) per thread when they fit: (32 + 2*32) heads * 8 slices = 768 threads at 7B
   int rope_threads = (((n_heads + 2 * n_kv_heads) * (head_dim / 16) + 31) / 32) * 32;
   rope_threads = rope_threads < 128 ? 128 : (rope_threads > 1024 ? 1024 : rope_threads);
-  LADE_CUDA_CHECK(launch_pdl(rope_append_kernel<T>, dim3(rows), dim3(rope_threads), 0, (cudaStream_t)stream,
+  LADE_CUDA_CHECK(launch_pdl(rope_append_kernel<T, QKNORM>, dim3(rows), dim3(rope_threads), 0, (cudaStream_t)stream,
                              (const T*)qkv, (const T*)cos_tab, (const T*)sin_tab, (const int*)pos, (const int*)meta,
                              (T*)q_out, (T*)k_cache, (T*)v_cache, q_pad, n_heads, n_kv_heads, head_dim, kv_capacity,
-                             max_pos));
+                             max_pos, (const T*)q_norm_w, (const T*)k_norm_w, eps));
   return LADE_OK;
 }
 
@@ -453,6 +492,22 @@ int lade_rope_append_f16(void* stream, const void* qkv, const void* cos_tab, con
                          int32_t kv_capacity, int32_t max_pos) {
   return rope_append_impl<__half>(stream, qkv, cos_tab, sin_tab, pos, meta, q_out, k_cache, v_cache, rows, q_pad,
                                   n_heads, n_kv_heads, head_dim, kv_capacity, max_pos);
+}
+int lade_rope_append_qknorm(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab,
+                            const int32_t* pos, const int32_t* meta, void* q_out, void* k_cache, void* v_cache,
+                            int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
+                            int32_t kv_capacity, int32_t max_pos, const void* q_norm_w, const void* k_norm_w, float eps) {
+  return rope_append_impl<__nv_bfloat16, true>(stream, qkv, cos_tab, sin_tab, pos, meta, q_out, k_cache, v_cache, rows,
+                                               q_pad, n_heads, n_kv_heads, head_dim, kv_capacity, max_pos, q_norm_w,
+                                               k_norm_w, eps);
+}
+int lade_rope_append_qknorm_f16(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab,
+                                const int32_t* pos, const int32_t* meta, void* q_out, void* k_cache, void* v_cache,
+                                int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
+                                int32_t kv_capacity, int32_t max_pos, const void* q_norm_w, const void* k_norm_w,
+                                float eps) {
+  return rope_append_impl<__half, true>(stream, qkv, cos_tab, sin_tab, pos, meta, q_out, k_cache, v_cache, rows, q_pad,
+                                        n_heads, n_kv_heads, head_dim, kv_capacity, max_pos, q_norm_w, k_norm_w, eps);
 }
 int lade_swiglu(void* stream, const void* gate_up, void* out, int32_t rows, int32_t inter) {
   return swiglu_impl<__nv_bfloat16>(stream, gate_up, out, rows, inter);

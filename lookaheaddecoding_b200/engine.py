@@ -1,6 +1,7 @@
 """Host-side driver of the H100 lookahead/verification step.
 
-One ``LookaheadEngine`` wraps one HF ``LlamaForCausalLM`` on one GPU.  Per decoding step it launches
+One ``LookaheadEngine`` wraps one HF ``LlamaForCausalLM`` (or ``Qwen3ForCausalLM``, whose per-head q/k RMSNorm
+runs inside ``lade_rope_append_qknorm``) on one GPU.  Per decoding step it launches
 (through the C-ABI of ``include/lade_sm100.h``):
 
     lade_step_layout -> embedding gather -> L x [ lade_rmsnorm -> QKV GEMM -> lade_rope_append ->
@@ -84,7 +85,8 @@ def processors_record(processors: dict) -> _cabi.LadeProcessors:
 
 
 class LookaheadEngine:
-    """Device-resident lookahead decoding for one Llama model (batch 1, bf16, CUDA)."""
+    """Device-resident lookahead decoding for one Llama-shaped model (batch 1, bf16 or fp16, CUDA): Llama, or Qwen3 with
+    its per-head q/k RMSNorm."""
 
     def __init__(self, model, window_size: int, level: int, guess_set_size: int,
                  pool_from_prompt: bool = False, max_total_len: int = 4096, attn_impl: int = 0,
@@ -104,6 +106,7 @@ class LookaheadEngine:
         self.k_rmsnorm = getattr(self.lib, "lade_rmsnorm" + sfx)
         self.k_rmsnorm_gather = getattr(self.lib, "lade_rmsnorm_gather" + sfx)
         self.k_rope_append = getattr(self.lib, "lade_rope_append" + sfx)
+        self.k_rope_append_qknorm = getattr(self.lib, "lade_rope_append_qknorm" + sfx)
         self.k_swiglu = getattr(self.lib, "lade_swiglu" + sfx)
         self.k_argmax_rows = getattr(self.lib, "lade_argmax_rows" + sfx)
         self.k_argmax_processed = getattr(self.lib, "lade_argmax_processed" + sfx)
@@ -142,6 +145,7 @@ class LookaheadEngine:
             raise LadeError(f"rope scaling '{rope_type}' is not supported (only the default rotary embedding)")
         self.rope_theta = float(rp.get("rope_theta", getattr(cfg, "rope_theta", 10000.0)) if isinstance(rp, dict)
                                 else getattr(cfg, "rope_theta", 10000.0))
+        self._check_attention_layout(model, int(max_total_len))
         self.attn_impl = attn_impl
         self.use_cuda_graph = use_cuda_graph
         self.lm_cap = 1 + self.WCAP + self.G * self.GS
@@ -206,6 +210,42 @@ class LookaheadEngine:
         self.last_records: List[StepRecord] = []
 
     # ------------------------------------------------------------------------------------------
+    def _check_attention_layout(self, model, max_total_len: int) -> None:
+        """Per-head q/k RMSNorm (Qwen3Attention: q_norm / k_norm in front of the rotary embedding) and sliding-window
+        layers.  A model with both norms on every layer, each of weight [head_dim], runs with the norms fused into the
+        RoPE kernel; any other shape of them, or a layer HF would run with a sliding window shorter than the engine's
+        capacity, is refused here, before anything is allocated: decoding it with the Llama step would be wrong."""
+        cfg = model.config
+        layer_types = getattr(cfg, "layer_types", None) or ()
+        window = getattr(cfg, "sliding_window", None)
+        if "sliding_attention" in layer_types and window is not None and int(window) < max_total_len:
+            raise LadeError(f"sliding-window attention (sliding_window={window} < max_total_len={max_total_len} on "
+                            f"{list(layer_types).count('sliding_attention')} layers) is not supported")
+        self.q_norm_w: Optional[List[torch.Tensor]] = None
+        self.k_norm_w: Optional[List[torch.Tensor]] = None
+        self.qk_eps: List[float] = []
+        found = [(getattr(l.self_attn, "q_norm", None), getattr(l.self_attn, "k_norm", None)) for l in model.model.layers]
+        if all(q is None and k is None for q, k in found):
+            return
+        qw, kw = [], []
+        for li, (qn, kn) in enumerate(found):
+            if qn is None or kn is None:
+                raise LadeError(f"layer {li} has {'k_norm' if qn is None else 'q_norm'} without "
+                                f"{'q_norm' if qn is None else 'k_norm'}: not supported")
+            for name, m_ in (("q_norm", qn), ("k_norm", kn)):
+                w = getattr(m_, "weight", None)
+                if w is None or tuple(w.shape) != (self.D,) or w.dtype != self.dt or not w.is_contiguous() \
+                        or not hasattr(m_, "variance_epsilon"):
+                    raise LadeError(f"layer {li} {name} ({type(m_).__name__}, weight "
+                                    f"{None if w is None else (tuple(w.shape), w.dtype)}) is not an RMSNorm over each "
+                                    f"head of {self.D} in {self.dt}: only per-head q/k norms (Qwen3) are supported")
+            if float(qn.variance_epsilon) != float(kn.variance_epsilon):
+                raise LadeError(f"layer {li}: q_norm and k_norm have different eps: not supported")
+            qw.append(qn.weight)
+            kw.append(kn.weight)
+            self.qk_eps.append(float(qn.variance_epsilon))
+        self.q_norm_w, self.k_norm_w = qw, kw
+
     def _fuse_weights(self):
         """Fuse q/k/v and gate/up into single GEMM operands; re-point the HF parameters at views of
         the fused storage so no second copy of the weights stays resident."""
@@ -364,7 +404,7 @@ class LookaheadEngine:
             kc, vc = self.kv[l, 0], self.kv[l, 1]
             n += self._norm(stream, h, delta, self.ln1[l], xn, rows)
             n += self._proj(xn, self.w_qkv[l], qkv)
-            n += self._rope_append(stream, qkv, qb, kc, vc, rows)
+            n += self._rope_append(stream, l, qkv, qb, kc, vc, rows)
             n += self._attention(stream, l, qb, kc, vc, attn_out, rows, prefill)
             n += self._proj(attn_out, self.w_o[l], o_buf)
             n += self._norm(stream, h, o_buf, self.ln2[l], xn, rows)
@@ -395,11 +435,16 @@ class LookaheadEngine:
         torch.mm(x, w.t(), out=out)
         return 0
 
-    def _rope_append(self, stream: int, qkv, qb, kc, vc, rows: int) -> int:
-        """RoPE on q and k; q to the head-major `qb`, k and v appended to the layer's cache."""
-        check(self.k_rope_append(stream, _ptr(qkv), _ptr(self.cos), _ptr(self.sin), _ptr(self.pos), _ptr(self.meta),
-                                 _ptr(qb), _ptr(kc), _ptr(vc), rows, rows, self.nh, self.nkv, self.D,
-                                 self.kv_capacity, self.table_len), "lade_rope_append")
+    def _rope_append(self, stream: int, l: int, qkv, qb, kc, vc, rows: int) -> int:
+        """RoPE on q and k of layer `l` (after their per-head RMSNorm on a model that has one); q to the head-major `qb`,
+        k and v appended to the layer's cache."""
+        args = (stream, _ptr(qkv), _ptr(self.cos), _ptr(self.sin), _ptr(self.pos), _ptr(self.meta), _ptr(qb), _ptr(kc),
+                _ptr(vc), rows, rows, self.nh, self.nkv, self.D, self.kv_capacity, self.table_len)
+        if self.q_norm_w is None:
+            check(self.k_rope_append(*args), "lade_rope_append")
+        else:
+            check(self.k_rope_append_qknorm(*args, _ptr(self.q_norm_w[l]), _ptr(self.k_norm_w[l]), self.qk_eps[l]),
+                  "lade_rope_append_qknorm")
         return 1
 
     def _attention(self, stream: int, l: int, qb, kc, vc, out, rows: int, prefill: bool) -> int:
