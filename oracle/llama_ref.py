@@ -31,7 +31,7 @@ def init_weights(cfg: dict, seed: int = 0, dtype=torch.float32) -> Dict[str, tor
     """
     H, L, I, V = cfg["hidden"], cfg["layers"], cfg["inter"], cfg["vocab"]
     nh, nkv = cfg["heads"], cfg.get("kv_heads") or cfg["heads"]
-    D = H // nh
+    D = cfg.get("head_dim") or H // nh
     shapes = {"lm_head.weight": (V, H), "model.embed_tokens.weight": (V, H), "model.norm.weight": (H,)}
     for i in range(L):
         p = f"model.layers.{i}."
@@ -55,18 +55,29 @@ def init_weights(cfg: dict, seed: int = 0, dtype=torch.float32) -> Dict[str, tor
     return w
 
 
-def rope_tables(D: int, max_pos: int, theta: float, dtype, device) -> Tuple[torch.Tensor, torch.Tensor]:
-    """cos/sin caches as modeling_llama.py:240-256 (fp32 math, then cast to the model dtype :264-265)."""
+def rope_tables(D: int, max_pos: int, theta: float, dtype, device,
+                table_dtype=None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """cos/sin caches as modeling_llama.py:240-256 (fp32 math, then cast to the model dtype :264-265).
+
+    `table_dtype` (default `dtype`) is the precision the tables are rounded to before they are widened to `dtype`: a
+    float64 forward takes either the tables a 16-bit model uses (the device step's operands) or the fp32 ones that HF
+    computes for a float64 model."""
     inv_freq = 1.0 / (theta ** (torch.arange(0, D, 2).float() / D))
     t = torch.arange(max_pos, dtype=inv_freq.dtype)
     freqs = torch.outer(t, inv_freq)
     emb = torch.cat((freqs, freqs), dim=-1)
-    return emb.cos().to(dtype).to(device), emb.sin().to(dtype).to(device)
+    td = dtype if table_dtype is None else table_dtype
+    return emb.cos().to(td).to(dtype).to(device), emb.sin().to(td).to(dtype).to(device)
+
+
+def _acc_dtype(dtype):
+    """Where the reference computes in fp32 (RMSNorm statistics, softmax): fp32, or float64 for a float64 forward."""
+    return torch.float64 if dtype == torch.float64 else torch.float32
 
 
 def rms_norm(x: torch.Tensor, w: torch.Tensor, eps: float) -> torch.Tensor:
     dt = x.dtype
-    xf = x.to(torch.float32)
+    xf = x.to(_acc_dtype(dt))
     var = xf.pow(2).mean(-1, keepdim=True)
     xf = xf * torch.rsqrt(var + eps)
     return w * xf.to(dt)
@@ -96,7 +107,7 @@ def eager_attention(q, k, v, mask, n_rep: int = 1):
     D = q.shape[-1]
     s = torch.matmul(q, k.transpose(1, 2)) / math.sqrt(D)
     s = s + mask
-    p = torch.nn.functional.softmax(s, dim=-1, dtype=torch.float32).to(q.dtype)
+    p = torch.nn.functional.softmax(s, dim=-1, dtype=_acc_dtype(q.dtype)).to(q.dtype)
     return torch.matmul(p, v)
 
 
@@ -298,20 +309,31 @@ def unexplained(got: torch.Tensor, main: torch.Tensor, alt: torch.Tensor) -> Tup
 
 
 class OracleLlama:
-    """Functional Llama with a growing KV cache, driven by ``oracle.lookahead.greedy_lookahead``."""
+    """Functional Llama with a growing KV cache, driven by ``oracle.lookahead.greedy_lookahead``.
 
-    def __init__(self, cfg: dict, weights: Dict[str, torch.Tensor], device="cpu"):
+    Qwen3 too: `cfg["head_dim"]` when heads * head_dim != hidden, and the per-head q/k RMSNorm in front of RoPE
+    (Qwen3Attention) when the weights hold ``self_attn.q_norm.weight`` / ``k_norm.weight``.
+
+    bf16 / fp16 weights give the reference's rounding points.  float64 weights give a float64 forward with no fp32
+    step inside (RMSNorm statistics, softmax and logits stay float64); it needs `rope_dtype`, the precision of its
+    RoPE tables: the model dtype of the 16-bit model it stands for (the device step's tables), or torch.float32
+    (HF's tables for a float64 model)."""
+
+    def __init__(self, cfg: dict, weights: Dict[str, torch.Tensor], device="cpu", rope_dtype=None):
         self.cfg = cfg
         self.dev = torch.device(device)
         self.w = {k: v.to(self.dev) for k, v in weights.items()}
         self.dtype = self.w["lm_head.weight"].dtype
+        if self.dtype == torch.float64 and rope_dtype is None:
+            raise ValueError("a float64 OracleLlama needs rope_dtype (the model dtype's tables or torch.float32)")
         self.H, self.L = cfg["hidden"], cfg["layers"]
         self.nh = cfg["heads"]
         self.nkv = cfg.get("kv_heads") or cfg["heads"]
-        self.D = self.H // self.nh
+        self.D = cfg.get("head_dim") or self.H // self.nh
         self.eps = cfg.get("eps", 1e-5)
+        self.qk_norm = "model.layers.0.self_attn.q_norm.weight" in self.w
         self.cos, self.sin = rope_tables(self.D, cfg.get("max_pos", 4096), cfg.get("rope_theta", 10000.0),
-                                         self.dtype, self.dev)
+                                         self.dtype, self.dev, table_dtype=rope_dtype)
         self.reset()
 
     def reset(self):
@@ -320,7 +342,7 @@ class OracleLlama:
         self.last_hidden = None
         self.last_attn_io = None
 
-    # -- one forward over the step rows, returns fp32 logits [q, V] -------------------------------
+    # -- one forward over the step rows, returns fp32 logits [q, V] (float64 for a float64 model) ---
     def forward_rows(self, ids, pos, vis_mask: torch.Tensor, kv_len: int, capture_layer: int = -1):
         w, dt = self.w, self.dtype
         ids_t = torch.as_tensor(ids, dtype=torch.long, device=self.dev)
@@ -336,6 +358,9 @@ class OracleLlama:
             q = torch.nn.functional.linear(x, w[p + "self_attn.q_proj.weight"]).view(q_len, self.nh, self.D).transpose(0, 1)
             k = torch.nn.functional.linear(x, w[p + "self_attn.k_proj.weight"]).view(q_len, self.nkv, self.D).transpose(0, 1)
             v = torch.nn.functional.linear(x, w[p + "self_attn.v_proj.weight"]).view(q_len, self.nkv, self.D).transpose(0, 1)
+            if self.qk_norm:                    # Qwen3RMSNorm over each head, before the rotary embedding
+                q = rms_norm(q, w[p + "self_attn.q_norm.weight"], self.eps)
+                k = rms_norm(k, w[p + "self_attn.k_norm.weight"], self.eps)
             q = (q * cos) + (rotate_half(q) * sin)
             k = (k * cos) + (rotate_half(k) * sin)
             if self.k_cache[i] is not None and kv_len > 0:
@@ -354,7 +379,8 @@ class OracleLlama:
             h = res + torch.nn.functional.linear(torch.nn.functional.silu(g) * u, w[p + "mlp.down_proj.weight"])
         h = rms_norm(h, w["model.norm.weight"], self.eps)
         self.last_hidden = h
-        return torch.nn.functional.linear(h, w["lm_head.weight"]).float()
+        logits = torch.nn.functional.linear(h, w["lm_head.weight"])
+        return logits if dt == torch.float64 else logits.float()
 
     # -- StepFn / CompactFn for oracle.lookahead.greedy_lookahead ---------------------------------
     def step_fn(self, lay: LA.StepLayout, kv_len: int):
