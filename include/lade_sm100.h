@@ -411,6 +411,27 @@ int lade_sample_verify_warped_f16(LadeCtx* ctx, void* stream, const void* logits
 int lade_commit_decision(LadeCtx* ctx, void* stream, const int32_t* decision, const int32_t* meta,
                          int32_t* result);
 
+/* Per-token logits capture (return_dict_in_generate with output_logits / output_scores, which the reference refuses,
+ * lade/decoding.py:411, :967).  Launched after the step's commit (lade_accept_update or lade_commit_decision) on the
+ * same stream, inside the same CUDA graph: for each token j the step emitted, the lm slot row it was decided from,
+ * logits[slot][0:vocab] (bf16; _f16: fp16), is copied to out[r][0:vocab], r = n_out_before - n_prompt + j, where
+ * n_out_before = result[LADE_R_N_OUT] - result[LADE_R_N_EMIT] and n_prompt is the prompt length of lade_ctx_reset: row r
+ * of `out` is generated token r.  Slot of token j: 0 for j = 0; for j >= 1 the verification slot (e, j-1) of n-gram
+ * e = result[LADE_R_MAX_HIT_IDX] when `sampling` is 0 (greedy: lade_accept_update emits the argmax of those slots), and
+ * e = the lowest-index n-gram whose tokens 0..j-1 equal hits[0..j-1] when `sampling` is 1 (the row the sampling chain
+ * drew token j from: the first candidate carrying each accepted token is the one that accepted it).  The n-grams'
+ * tokens are read from the step's rows, ids[lm_rows[slot]] (lade_step_layout of the same step).  Writes nothing when
+ * the step ran on a finished state (meta[LADE_M_DONE]) or emitted nothing, and never a row >= out_rows.  Rows are
+ * `ld` / `ld_out` elements apart (>= vocab); 16-byte copies where both rows allow them.  LADE_EINVAL for a null
+ * pointer, vocab < 1, ld or ld_out < vocab, out_rows < 1, `sampling` not 0 or 1, a pointer not aligned to its element
+ * (nothing is launched); LADE_EUNSUPPORTED for a lookahead-parallel ctx. */
+int lade_capture_rows(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab, const int32_t* ids,
+                      const int32_t* lm_rows, const int32_t* meta, const int32_t* result, int32_t sampling, void* out,
+                      int32_t ld_out, int32_t out_rows);
+int lade_capture_rows_f16(LadeCtx* ctx, void* stream, const void* logits, int32_t ld, int32_t vocab, const int32_t* ids,
+                          const int32_t* lm_rows, const int32_t* meta, const int32_t* result, int32_t sampling,
+                          void* out, int32_t ld_out, int32_t out_rows);
+
 /* Move the accepted n-gram's K/V rows to the cache tail for every layer (lade/decoding.py:1156-1163): rows
  * [R_KV_SRC, R_KV_SRC + h) of every head go to [R_KV_DST, R_KV_DST + h), h = min(R_MAX_HIT, max_rows); nothing moves when
  * R_MAX_HIT is 0 or R_KV_SRC < 0.  k_base/v_base point at layer 0; layers are `layer_stride_elems` apart (at least

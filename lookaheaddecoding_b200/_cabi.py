@@ -80,6 +80,7 @@ _SIGNATURES = {
     "lade_sample_verify": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32, c_p, c_p, C.c_float, c_i32, C.c_float, c_p, c_p, c_p]),
     "lade_sample_verify_warped": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32, c_p, c_p, C.POINTER(LadeWarpers), c_p, c_p, c_p,
                                             c_p]),
+    "lade_capture_rows": (C.c_int, [c_p, c_p, c_p, c_i32, c_i32, c_p, c_p, c_p, c_p, c_i32, c_p, c_i32, c_i32]),
     "lade_kv_compact": (C.c_int, [c_p, c_p, c_p, c_p, C.c_int64, c_i32, c_i32, c_i32, c_i32, c_i32]),
     "lade_ctx_output_ids": (C.c_int, [c_p, c_p, c_p, c_i32]),
     "lade_ctx_pool_snapshot": (C.c_int, [c_p, c_p, c_p, c_p]),
@@ -100,7 +101,8 @@ _SIGNATURES = {
 # fp16 twins: same signatures as the bf16 entry points
 for _name in ("lade_rmsnorm", "lade_rmsnorm_gather", "lade_rope_append", "lade_rope_append_qknorm", "lade_swiglu",
               "lade_argmax_rows", "lade_attn_fwd", "lade_sample_verify", "lade_argmax_processed", "lade_sample_verify_warped",
-              "lade_gemm_fp8", "lade_rmsnorm_quant_fp8", "lade_swiglu_quant_fp8", "lade_quant_rows_fp8"):
+              "lade_gemm_fp8", "lade_rmsnorm_quant_fp8", "lade_swiglu_quant_fp8", "lade_quant_rows_fp8",
+              "lade_capture_rows"):
     _SIGNATURES[_name + "_f16"] = _SIGNATURES[_name]
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

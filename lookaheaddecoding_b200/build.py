@@ -16,7 +16,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_DIR = os.path.join(PKG_DIR, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "liblade_sm100.so")
 STAMP = os.path.join(LIB_DIR, "liblade_sm100.stamp")
-SOURCES = ["state.cu", "sampling.cu", "layer_ops.cu", "attn_mma.cu", "attn_tc.cu", "attn_api.cu", "gemm_tc.cu", "lp_nccl.cu"]
+SOURCES = ["state.cu", "sampling.cu", "capture.cu","layer_ops.cu", "attn_mma.cu", "attn_tc.cu", "attn_api.cu", "gemm_tc.cu", "lp_nccl.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC", "-ldl",

@@ -60,6 +60,7 @@ def sample_entry_proxy(self, input_ids, logits_processor=None, stopping_criteria
         output_attentions=bool(generation_config.output_attentions),
         output_hidden_states=bool(generation_config.output_hidden_states),
         output_scores=bool(generation_config.output_scores),
+        output_logits=bool(getattr(generation_config, "output_logits", False)),
         return_dict_in_generate=bool(generation_config.return_dict_in_generate),
         synced_gpus=synced_gpus, streamer=streamer, **model_kwargs)
     if do_sample:
@@ -144,6 +145,39 @@ def processors_from_hf(logits_processor) -> Optional[dict]:
     return out
 
 
+def check_output_options(output_attentions, output_hidden_states) -> None:
+    """The per-step outputs generate() cannot return: the step computes attention and hidden states for many rows at
+    once and keeps none of them per emitted token."""
+    if output_attentions or output_hidden_states:
+        raise LadeError("output_attentions / output_hidden_states are not supported on the lookahead path")
+
+
+def wants_logits(return_dict_in_generate, output_logits, output_scores) -> bool:
+    """Whether generate() has to capture the per-token logits rows (HF ignores output_logits / output_scores unless
+    return_dict_in_generate is set)."""
+    return bool(return_dict_in_generate and (output_logits or output_scores))
+
+
+def generate_output(sequences: torch.Tensor, n_prompt: int, rows: Optional[torch.Tensor], logits_processor,
+                    output_logits: bool, output_scores: bool):
+    """HF's ``GenerateDecoderOnlyOutput`` of a lookahead generate().  `rows` [generated, V] (model dtype) holds the row
+    each generated token was decided from; HF's ``logits`` are those rows in float32 and its ``scores`` the same rows
+    after `logits_processor` (the very objects HF built: processors, then warpers when sampling), each applied against
+    the token's own prefix ``sequences[:, :n_prompt + j]``.  Every processor the lookahead path accepts depends on
+    nothing but (prefix, row), so this is what HF's own loop computes from the same rows."""
+    from transformers.generation.utils import GenerateDecoderOnlyOutput
+    logits = scores = None
+    if rows is not None:
+        raw = tuple(rows[j:j + 1].float() for j in range(rows.shape[0]))
+        if output_logits:
+            logits = raw
+        if output_scores:
+            scores = tuple(logits_processor(sequences[:, :n_prompt + j], r.clone()) if logits_processor else r.clone()
+                           for j, r in enumerate(raw))
+    return GenerateDecoderOnlyOutput(sequences=sequences, scores=scores, logits=logits, attentions=None,
+                                     hidden_states=None, past_key_values=None)
+
+
 def get_engine(model, **overrides) -> LookaheadEngine:
     """One engine per (model, lookahead config); reads CONFIG_MAP like lade/decoding.py:854-862."""
     W = CONFIG_MAP.get("WINDOW_SIZE", 60)
@@ -176,28 +210,29 @@ def get_engine(model, **overrides) -> LookaheadEngine:
 def jacobi_greedy_search_multilevel(self, input_ids: torch.LongTensor, logits_processor=None,
                                     stopping_criteria=None, max_length: Optional[int] = None,
                                     pad_token_id=None, eos_token_id=None, output_attentions=None,
-                                    output_hidden_states=None, output_scores=None,
+                                    output_hidden_states=None, output_scores=None, output_logits=None,
                                     return_dict_in_generate=None, synced_gpus: bool = False, streamer=None,
                                     chat: bool = False, stop_token: Optional[str] = None, **model_kwargs):
     """Greedy lookahead decoding on the H100 engine; drop-in for lade/decoding.py:697-1259.
 
     Logits processors: the prefix-only ones of ``processors_from_hf`` run on device (the reference allows none,
-    :968); any other raises.  Inherited restrictions (fail loudly, as the reference asserts): batch size 1
-    (modeling_llama.py:1448), ``return_dict_in_generate == False``
-    (:967), ``ALWAYS_FWD_ONE == 1`` (:873), LEVEL >= 3 (:902).  ``stop_token`` / ``chat`` are
-    accepted and ignored (UI only).
+    :968); any other raises.  ``return_dict_in_generate=True`` (which the reference refuses, :967) returns HF's
+    ``GenerateDecoderOnlyOutput``; with ``output_logits`` / ``output_scores`` the rows the engine decided each token
+    from are captured on device (``generate_output``).  Inherited restrictions (fail loudly, as the reference asserts):
+    batch size 1 (modeling_llama.py:1448), ``ALWAYS_FWD_ONE == 1`` (:873), LEVEL >= 3 (:902); no
+    ``output_attentions`` / ``output_hidden_states``.  ``stop_token`` / ``chat`` are accepted and ignored (UI only).
     """
     if input_ids.shape[0] != 1:
         raise LadeError("lookahead decoding supports batch size 1 only (modeling_llama.py:1448)")
     processors = processors_from_hf(logits_processor)
     if processors and CONFIG_MAP.get("DIST_WORKERS", 1) > 1:
         raise LadeError("logits processors are not supported with lookahead parallelism (DIST_WORKERS > 1)")
-    if return_dict_in_generate:
-        raise LadeError("return_dict_in_generate must be False (decoding.py:967)")
     if CONFIG_MAP.get("ALWAYS_FWD_ONE", 1) != 1:
         raise LadeError("ALWAYS_FWD_ONE must be 1 (decoding.py:873)")
-    if output_attentions or output_hidden_states or output_scores:
-        raise LadeError("output_attentions/hidden_states/scores are not supported")
+    check_output_options(output_attentions, output_hidden_states)
+    capture = wants_logits(return_dict_in_generate, output_logits, output_scores)
+    if capture and CONFIG_MAP.get("DIST_WORKERS", 1) > 1:
+        raise LadeError("output_logits / output_scores are not supported with lookahead parallelism (DIST_WORKERS > 1)")
     if isinstance(eos_token_id, int):
         eos_token_id = [eos_token_id]                                          # decoding.py:820-821
     if torch.is_tensor(eos_token_id):
@@ -210,7 +245,7 @@ def jacobi_greedy_search_multilevel(self, input_ids: torch.LongTensor, logits_pr
     prompt = input_ids[0].tolist()
     stop_fn = _host_stop_fn(_extra_stopping_criteria(stopping_criteria), input_ids.device, input_ids.dtype)
     out = eng.generate(prompt, total - init_len, eos_token_ids=eos_token_id or (), rng=random, stop_fn=stop_fn,
-                       processors=processors)
+                       processors=processors, capture_logits=capture)
     if streamer is not None:
         streamer.put(torch.tensor(out[init_len:]))
         streamer.end()
@@ -220,4 +255,8 @@ def jacobi_greedy_search_multilevel(self, input_ids: torch.LongTensor, logits_pr
         print("Generated tokens: ", n_gen, "Total steps: ", steps, " Compression ratio: ", round(n_gen / steps, 2))
         print("======================================================================================", end="")
         CONFIG_MAP.setdefault("log", []).append([n_gen, steps, round(n_gen / steps, 2)])
-    return torch.tensor([out], dtype=input_ids.dtype, device=input_ids.device)
+    sequences = torch.tensor([out], dtype=input_ids.dtype, device=input_ids.device)
+    if return_dict_in_generate:
+        return generate_output(sequences, init_len, eng.last_logits if capture else None, logits_processor,
+                               bool(output_logits), bool(output_scores))
+    return sequences

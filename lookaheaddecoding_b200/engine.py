@@ -7,7 +7,7 @@ runs inside ``lade_rope_append_qknorm``) on one GPU.  Per decoding step it launc
     lade_step_layout -> embedding gather -> L x [ lade_rmsnorm -> QKV GEMM -> lade_rope_append ->
     lade_attn_fwd -> O GEMM -> lade_rmsnorm(+residual) -> gate/up GEMM -> lade_swiglu -> down GEMM ]
     -> lade_rmsnorm_gather (live lm_head rows only) -> lm_head GEMM -> lade_argmax_rows ->
-    lade_accept_update -> lade_kv_compact
+    lade_accept_update -> lade_kv_compact [-> lade_capture_rows, with capture_logits]
 
 which is the GPU re-design of one iteration of the reference's ``while True`` loop
 (``lade/decoding.py:923-1219``) including ``jforward_multilevel``
@@ -84,6 +84,28 @@ def processors_record(processors: dict) -> _cabi.LadeProcessors:
     return r
 
 
+def first_matching_candidate(guess_tokens: Sequence[int], gs: int, hits: Sequence[int], i: int) -> int:
+    """The candidate the sampling verification accepted at position i: the lowest-index n-gram whose tokens 0..i equal
+    hits[0..i] (an earlier n-gram carrying hits[i] would have been tested first, and its rejection zeroes that token
+    for every later one), or -1 when none does (hits[i] was drawn, not accepted)."""
+    for e in range(len(guess_tokens) // gs):
+        if all(guess_tokens[e * gs + u] == hits[u] for u in range(i + 1)):
+            return e
+    return -1
+
+
+def decided_slots(n_emit: int, hits: Sequence[int], window_cap: int, gs: int, sampling: bool, max_hit_idx: int = 0,
+                  guess_tokens: Sequence[int] = ()) -> List[int]:
+    """The lm slot each of a step's n_emit emitted tokens was decided from (what lade_capture_rows copies): slot 0 for
+    the first; for token j >= 1 the verification slot (e, j-1), with e = max_hit_idx on the greedy path and the first
+    matching candidate at position j-1 on the sampling path."""
+    slots = [0] if n_emit > 0 else []
+    for j in range(1, n_emit):
+        e = first_matching_candidate(guess_tokens, gs, hits, j - 1) if sampling else max_hit_idx
+        slots.append(1 + window_cap + e * gs + j - 1)
+    return slots
+
+
 class LookaheadEngine:
     """Device-resident lookahead decoding for one Llama-shaped model (batch 1, bf16 or fp16, CUDA): Llama, or Qwen3 with
     its per-head q/k RMSNorm."""
@@ -113,6 +135,7 @@ class LookaheadEngine:
         self.k_attn_fwd = getattr(self.lib, "lade_attn_fwd" + sfx)
         self.k_sample_verify = getattr(self.lib, "lade_sample_verify" + sfx)
         self.k_sample_verify_warped = getattr(self.lib, "lade_sample_verify_warped" + sfx)
+        self.k_capture_rows = getattr(self.lib, "lade_capture_rows" + sfx)
         if level < 3:
             raise LadeError("LEVEL must be >= 3 (lade/decoding.py:902)")
         if guess_set_size == -1:
@@ -206,6 +229,11 @@ class LookaheadEngine:
         self.debug_uniforms: Optional[torch.Tensor] = None
         # tests set a device float[>= 1 + 2*(N-1)]: lade_sample_verify_warped then records each visited row's cut
         self.debug_cuts: Optional[torch.Tensor] = None
+        # logits capture of the current generate() (capture_logits=True): [rows][V] in the model dtype, row r = the lm
+        # row generated token r was decided from (lade_capture_rows after every step's commit)
+        self.capture_on = False
+        self.capture_buf: Optional[torch.Tensor] = None
+        self.last_logits: Optional[torch.Tensor] = None
         self.last_steps = 0
         self.last_records: List[StepRecord] = []
 
@@ -422,7 +450,8 @@ class LookaheadEngine:
             check(self.k_argmax_rows(stream, _ptr(self.logits), self.lm_cap, self.V, self.V, _ptr(self.am)),
                   "lade_argmax_rows")
         n += 1
-        return n + self._commit(stream, commit)
+        n += self._commit(stream, commit)
+        return n + self._capture(stream, commit)
 
     def _norm(self, stream: int, h, delta, w, out, rows: int) -> int:
         """out = rmsnorm(h + delta) * w; with a delta the residual sum is also written back to h."""
@@ -501,6 +530,17 @@ class LookaheadEngine:
               "lade_kv_compact")
         return n + 1
 
+    def _capture(self, stream: int, commit) -> int:
+        """With capture on, copy the row each token the step emitted was decided from into capture_buf (after the
+        commit has written res).  Off, or on a step the host decides (commit=False), nothing is launched."""
+        if not (self.capture_on and commit):
+            return 0
+        buf = self.capture_buf
+        check(self.k_capture_rows(self._ctx, stream, _ptr(self.logits), self.V, self.V, _ptr(self.ids),
+                                  _ptr(self.lm_rows), _ptr(self.meta), _ptr(self.res), int(commit == "sample"),
+                                  _ptr(buf), buf.stride(0), buf.shape[0]), "lade_capture_rows")
+        return 1
+
     def _cuts_on(self) -> bool:
         """Any of MinP / epsilon / eta set: the sampling step runs lade_sample_verify_warped."""
         return bool(self.sample_min_p or self.sample_epsilon or self.sample_eta)
@@ -569,6 +609,8 @@ class LookaheadEngine:
         key = (commit, float(self.sample_temperature), int(self.sample_top_k), float(self.sample_top_p),
                float(self.sample_min_p), float(self.sample_epsilon), float(self.sample_eta)) \
             if commit == "sample" else (commit, self.processors_on)
+        if self.capture_on:       # the capture launch bakes the buffer in: one graph per buffer
+            key = key + (("capture", self.capture_buf.data_ptr(), self.capture_buf.shape[0]),)
         if key in self._graph:
             self._graph_n = self._graph[key][1]
             return self._graph[key][0]
@@ -599,10 +641,20 @@ class LookaheadEngine:
             self._steady_graph(commit).replay()
             self.launches += self._graph_n
 
-    def begin(self, prompt, max_length: int, eos_token_ids, window0, processors: Optional[dict] = None) -> None:
+    def begin(self, prompt, max_length: int, eos_token_ids, window0, processors: Optional[dict] = None,
+              capture_logits: bool = False) -> None:
         """Reset the device state for a generate() call (lade_ctx_reset), write the logits-processor record and size
-        the buffers."""
+        the buffers.  `capture_logits`: every step also copies the rows its tokens were decided from into capture_buf,
+        max_length - P + N - 1 rows (a step may emit up to N - 2 tokens past max_length)."""
         P = len(prompt)
+        if capture_logits and self.DW != 1:
+            raise LadeError("logits capture is not supported with lookahead parallelism (DIST_WORKERS > 1): the "
+                            "accepted n-gram's rows live on one rank")
+        self.capture_on = bool(capture_logits)
+        if self.capture_on:
+            rows = max_length - P + self.GS
+            if self.capture_buf is None or self.capture_buf.shape[0] < rows:
+                self.capture_buf = torch.empty(rows, self.V, dtype=self.dt, device=self.dev)
         rec = processors_record(processors) if processors else None
         self._ensure_ctx(eos_token_ids)
         stream = torch.cuda.current_stream(self.dev).cuda_stream
@@ -637,7 +689,8 @@ class LookaheadEngine:
     @torch.no_grad()
     def generate(self, prompt_ids: Sequence[int], max_new_tokens: int, eos_token_ids: Sequence[int] = (),
                  rng: Optional[random.Random] = None, window0: Optional[Sequence[int]] = None,
-                 stop_fn=None, sampling: Optional[dict] = None, processors: Optional[dict] = None) -> List[int]:
+                 stop_fn=None, sampling: Optional[dict] = None, processors: Optional[dict] = None,
+                 capture_logits: bool = False) -> List[int]:
         """Greedy lookahead decoding; returns prompt + generated ids (trimmed to P + max_new_tokens).
         `stop_fn(ids) -> bool`: host-evaluated stopping criteria beyond max-length / EOS, checked after every step
         like lade/decoding.py:1215 (disables the one-step-deep host pipelining).
@@ -650,7 +703,11 @@ class LookaheadEngine:
         (every key optional): HF's greedy RepetitionPenalty / NoRepeatNGram / MinLength logits processors, applied on
         device to every row the step's verification reads, each against the prefix that row stands for
         (lade_argmax_processed).  "min_length" is the length below which the eos ids score -inf
-        (max(min_length, prompt_length + min_new_tokens) for HF's two processors).  Greedy and one GPU only."""
+        (max(min_length, prompt_length + min_new_tokens) for HF's two processors).  Greedy and one GPU only.
+        `capture_logits=True`: afterwards `last_logits` is a [generated tokens, V] view (model dtype) whose row j is the
+        lm-head row generated token j was decided from -- the model's next-token logits for exactly that token's
+        prefix, since lookahead is lossless -- captured on device inside the step graph (lade_capture_rows); the next
+        capturing generate() reuses the buffer.  One GPU only."""
         prompt = [int(t) for t in prompt_ids]
         P = len(prompt)
         max_length = P + int(max_new_tokens)
@@ -679,7 +736,9 @@ class LookaheadEngine:
             self.sample_temperature, self.sample_top_k, self.sample_top_p = T, top_k, top_p
             self.sample_min_p, self.sample_epsilon, self.sample_eta = cuts
             commit = "sample"
-        self.begin(prompt, max_length, eos_token_ids, self.draw_window(prompt, rng, window0), processors)
+        self.last_logits = None
+        self.begin(prompt, max_length, eos_token_ids, self.draw_window(prompt, rng, window0), processors,
+                   capture_logits=capture_logits)
         if sampling is not None:
             self.rng_state.copy_(torch.tensor([int(sampling.get("seed", 0)) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64))
         stream = torch.cuda.current_stream(self.dev).cuda_stream
@@ -727,4 +786,6 @@ class LookaheadEngine:
             torch.cuda.current_stream(self.dev).synchronize()
             inflight.clear()
         self.last_steps = step
+        if self.capture_on:
+            self.last_logits = self.capture_buf[:len(out[:max_length]) - P]
         return out[:max_length]                                   # lade/decoding.py:1221-1225

@@ -16,7 +16,7 @@ Two ways to run the multi-candidate rejection-sampling verification (``decoding.
 
 Restrictions inherited from the reference: warpers within {Temperature, TopK, TopP} (``decoding.py:375-377``), to
 which this port adds the threshold warpers {MinP, Epsilon, Eta} (each keeps every score at or above a cut, so lookahead
-stays lossless: every verification row is warped as its own distribution, like the top-p cut); no other logits processors (``:412``), batch 1, ``return_dict_in_generate == False``; no lookahead
+stays lossless: every verification row is warped as its own distribution, like the top-p cut); no other logits processors (``:412``), batch 1, no ``output_attentions`` / ``output_hidden_states``; no lookahead
 parallelism on this path (the reference has none either beyond the initial window broadcast).
 """
 from __future__ import annotations
@@ -117,8 +117,10 @@ def device_temperature(logits_warper):
 
 @torch.no_grad()
 def sample_lookahead(eng, prompt: List[int], max_new_tokens: int, logits_warper, eos_token_ids=(),
-                     rng=None, window0=None, stop_fn=None) -> List[int]:
-    """Drive one sampling generate() on `eng` (a LookaheadEngine). Returns prompt + sampled ids."""
+                     rng=None, window0=None, stop_fn=None, capture_logits: bool = False) -> List[int]:
+    """Drive one sampling generate() on `eng` (a LookaheadEngine). Returns prompt + sampled ids.  `capture_logits`:
+    afterwards `eng.last_logits` holds, per generated token, the logits row it was decided from (slot 0, then the
+    verification row of each accepted candidate), gathered from `eng.logits` on the host side of the loop."""
     if eng.DW != 1:
         raise LadeError("the sampling path has no lookahead parallelism (reference: replicas only)")
     rnd = rng or random
@@ -148,6 +150,8 @@ def sample_lookahead(eng, prompt: List[int], max_new_tokens: int, logits_warper,
     next_tokens = None            # the reference's `next_tokens` is only refreshed on some branches (sic)
     step = 0
     eng.last_records = []
+    eng.last_logits = None
+    captured = []                 # per step: the rows its emitted tokens were decided from
     while True:
         eng.run_forward_step(step, P, commit=False)
         meta = eng.meta.cpu().tolist()                       # sync point (the reference has several per step)
@@ -157,6 +161,7 @@ def sample_lookahead(eng, prompt: List[int], max_new_tokens: int, logits_warper,
         next_token_logits = eng.logits[0:1].float()                                        # outputs.out_logits
         next_token_scores = warp(input_ids, next_token_logits)                             # :445
         max_hit, max_hit_idx = 0, 0
+        src_slots = [0]           # lm slot each hit is decided from: slot 0, then the row after each accepted token
         new_results = list(inp_tokens)
         filtered = None
         if phase != 2 or lg == 0:                                                          # :458-480, :543-546
@@ -191,6 +196,7 @@ def sample_lookahead(eng, prompt: List[int], max_new_tokens: int, logits_warper,
                 max_hit_idx = winner
                 alive &= grams[:, pos] == tok                                   # :513-516
                 dist = slot_probs[winner * GS + pos]                            # :530
+                src_slots.append(1 + WCAP + winner * GS + pos)
             max_hit = len(hits) - 1
         if phase == 2 and eos:                                                             # :578-580
             filtered = list(new_results)          # the pool was already fed the unfiltered row (:563)
@@ -228,6 +234,8 @@ def sample_lookahead(eng, prompt: List[int], max_new_tokens: int, logits_warper,
         check(lib.lade_kv_compact(stream, eng.res.data_ptr(), eng.kv[0, 0].data_ptr(), eng.kv[0, 1].data_ptr(),
                                   eng.kv.stride(0), eng.L, eng.nkv, eng.kv_capacity, eng.D, max(GS - 1, 1)), "lade_kv_compact")
         eng.launches += 2
+        if capture_logits:
+            captured.append(eng.logits[torch.tensor(src_slots[:n_emit], device=dev)])   # a copy: the next step rewrites
         rec = eng._read_result()
         eng.last_records.append(rec)
         out.extend(hits[:n_emit])
@@ -238,23 +246,29 @@ def sample_lookahead(eng, prompt: List[int], max_new_tokens: int, logits_warper,
         if step > max_new_tokens + N + 4:
             raise LadeError("sampling loop did not terminate")
     eng.last_steps = step
+    if capture_logits:
+        eng.last_logits = torch.cat(captured)[:len(out[:max_length]) - P]
     return out[:max_length]
 
 
 def jacobi_sample_multilevel(self, input_ids: torch.LongTensor, logits_processor=None, stopping_criteria=None,
                              logits_warper=None, max_length: Optional[int] = None, pad_token_id=None,
                              eos_token_id=None, output_attentions=None, output_hidden_states=None,
-                             output_scores=None, return_dict_in_generate=None, synced_gpus: bool = False,
-                             streamer=None, chat: bool = False, **model_kwargs):
-    """Drop-in for lade/decoding.py:137 (same argument meaning; `chat` accepted and ignored)."""
-    from .decoding import CONFIG_MAP, _max_length_from, get_engine
+                             output_scores=None, output_logits=None, return_dict_in_generate=None,
+                             synced_gpus: bool = False, streamer=None, chat: bool = False, **model_kwargs):
+    """Drop-in for lade/decoding.py:137 (same argument meaning; `chat` accepted and ignored).  Unlike the reference
+    (:411), ``return_dict_in_generate=True`` returns HF's ``GenerateDecoderOnlyOutput``, with ``logits`` / ``scores``
+    built from the rows each token was drawn or accepted from (``decoding.generate_output``; scores apply the
+    processors, then the warpers, as HF does)."""
+    from .decoding import CONFIG_MAP, _max_length_from, check_output_options, generate_output, get_engine, wants_logits
+    from transformers.generation.logits_process import LogitsProcessorList
 
     if input_ids.shape[0] != 1:
         raise LadeError("lookahead decoding supports batch size 1 only (modeling_llama.py:1448)")
     if logits_processor is not None and len(logits_processor) != 0:
         raise LadeError("logits processors are not supported (decoding.py:412)")
-    if return_dict_in_generate:
-        raise LadeError("return_dict_in_generate must be False (decoding.py:411)")
+    check_output_options(output_attentions, output_hidden_states)
+    capture = wants_logits(return_dict_in_generate, output_logits, output_scores)
     _check_warpers(logits_warper)
     if isinstance(eos_token_id, int):
         eos_token_id = [eos_token_id]
@@ -275,10 +289,10 @@ def jacobi_sample_multilevel(self, input_ids: torch.LongTensor, logits_processor
     if params is not None and not CONFIG_MAP.get("SAMPLING_ON_HOST", 0):
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())          # reproducible under torch.manual_seed
         out = eng.generate(input_ids[0].tolist(), total - init_len, eos_token_ids=eos_token_id or (), rng=random,
-                           stop_fn=stop_fn, sampling=dict(params, seed=seed))
+                           stop_fn=stop_fn, sampling=dict(params, seed=seed), capture_logits=capture)
     else:
         out = sample_lookahead(eng, input_ids[0].tolist(), total - init_len, logits_warper, eos_token_id or (), rng=random,
-                               stop_fn=stop_fn)
+                               stop_fn=stop_fn, capture_logits=capture)
     if streamer is not None:
         streamer.put(torch.tensor(out[init_len:]))
         streamer.end()
@@ -288,4 +302,9 @@ def jacobi_sample_multilevel(self, input_ids: torch.LongTensor, logits_processor
         print("Generated tokens: ", n_gen, "Total steps: ", steps, " Compression ratio: ", round(n_gen / steps, 2))
         print("======================================================================================", end="")
         CONFIG_MAP.setdefault("log", []).append([n_gen, steps, round(n_gen / steps, 2)])
-    return torch.tensor([out], dtype=input_ids.dtype, device=input_ids.device)
+    sequences = torch.tensor([out], dtype=input_ids.dtype, device=input_ids.device)
+    if return_dict_in_generate:
+        chain = LogitsProcessorList(list(logits_processor or []) + list(logits_warper or []))
+        return generate_output(sequences, init_len, eng.last_logits if capture else None, chain, bool(output_logits),
+                               bool(output_scores))
+    return sequences
