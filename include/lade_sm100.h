@@ -212,6 +212,25 @@ int lade_rope_append_qknorm_f16(void* stream, const void* qkv, const void* cos_t
                                 int32_t kv_capacity, int32_t max_pos, const void* q_norm_w, const void* k_norm_w,
                                 float eps);
 
+/* Qwen2 / Qwen2.5 variant (Qwen2ForCausalLM): q_proj, k_proj and v_proj carry a bias, added before the rotary
+ * embedding.  Qwen2Attention.forward (transformers modeling_qwen2.py):
+ *     query_states = self.q_proj(hidden_states).view(hidden_shape).transpose(1, 2)      (the same for k and v)
+ *     query_states, key_states = apply_rotary_pos_emb(query_states, key_states, cos, sin)
+ * nn.Linear with a bias is addmm: the bias is added to the fp32 accumulator and the sum is rounded once.  So `qkv` is
+ * here the fused projection's fp32 accumulator [rows][(Hq+2Hkv)*D] (float, 16-byte aligned), and every element is first
+ * x = T(acc + float(bias)); RoPE of lade_rope_append then runs on q and k, v is appended as x.  bias: device
+ * T[(Hq+2Hkv)*D], the three biases concatenated in qkv's column order, 16-byte aligned.  Arguments, layouts and
+ * errors otherwise as lade_rope_append; LADE_EINVAL also for a null or misaligned bias or qkv.  Nothing is launched on
+ * an error.  _f16: fp16 models. */
+int lade_rope_append_bias(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab,
+                          const int32_t* pos, const int32_t* meta, void* q_out, void* k_cache, void* v_cache,
+                          int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
+                          int32_t kv_capacity, int32_t max_pos, const void* bias);
+int lade_rope_append_bias_f16(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab,
+                              const int32_t* pos, const int32_t* meta, void* q_out, void* k_cache, void* v_cache,
+                              int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
+                              int32_t kv_capacity, int32_t max_pos, const void* bias);
+
 /* Lookahead attention over the persistent KV cache (the roofline kernel).  softmax(QK^T/sqrt(D) +
  * lookahead mask) V with the mask bits of `rowmask` tested in registers (prefill steps: plain causal,
  * rowmask unused); all step rows see the committed cache.  Replaces LlamaAttention.forward's attention core (modeling_llama.py:520-541), the

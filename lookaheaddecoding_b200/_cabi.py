@@ -61,6 +61,7 @@ _SIGNATURES = {
     "lade_rmsnorm_gather": (C.c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_i32, c_i32, C.c_float]),
     "lade_rope_append": (C.c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p] + [c_i32] * 7),
     "lade_rope_append_qknorm": (C.c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p] + [c_i32] * 7 + [c_p, c_p, C.c_float]),
+    "lade_rope_append_bias": (C.c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p] + [c_i32] * 7 + [c_p]),
     "lade_attn_fwd": (C.c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_i32, c_p, c_p] + [c_i32] * 8),
     "lade_attn_scratch_bytes": (C.c_int64, [c_i32, c_i32, c_i32, c_i32]),
     "lade_debug_attn_timing": (C.c_int, [c_p]),
@@ -99,7 +100,8 @@ _SIGNATURES = {
 }
 
 # fp16 twins: same signatures as the bf16 entry points
-for _name in ("lade_rmsnorm", "lade_rmsnorm_gather", "lade_rope_append", "lade_rope_append_qknorm", "lade_swiglu",
+for _name in ("lade_rmsnorm", "lade_rmsnorm_gather", "lade_rope_append", "lade_rope_append_qknorm",
+              "lade_rope_append_bias", "lade_swiglu",
               "lade_argmax_rows", "lade_attn_fwd", "lade_sample_verify", "lade_argmax_processed", "lade_sample_verify_warped",
               "lade_gemm_fp8", "lade_rmsnorm_quant_fp8", "lade_swiglu_quant_fp8", "lade_quant_rows_fp8",
               "lade_capture_rows"):

@@ -2,6 +2,7 @@
 //   RMSNorm (+ fused residual add)   lade/models/modeling_llama.py:222-227, :883-889
 //   rotary embedding + KV append     lade/models/modeling_llama.py:342-346, :513-516
 //   (Qwen3: per-head q/k RMSNorm in front of the rotary embedding, fused into the same kernel)
+//   (Qwen2 / 2.5: the q/k/v projection biases added to the fp32 projection in the same kernel)
 //   SwiGLU                            lade/models/modeling_llama.py:378
 // All are HBM-bound byte movers: 16-byte vectorised, coalesced, one pass over the data.
 //
@@ -15,6 +16,7 @@
 #include <cuda_fp8.h>
 
 #include <cstdlib>
+#include <type_traits>
 
 namespace lade {
 
@@ -205,13 +207,32 @@ __global__ void __launch_bounds__(1024) rmsnorm_kernel(const T* __restrict__ x,
 // squares is a shuffle reduction inside that lane group.  A group enters or leaves the loop, the V branch and the
 // capacity test as a whole (n_items is a multiple of D/16; the other two depend on the head and the row only), so
 // every lane of the group's shuffle mask reaches the shuffle.
-template <typename T, bool QKNORM>
+// TIN = float (Qwen2Attention.forward: q_proj / k_proj / v_proj carry a bias): qkv is the projection's fp32 accumulator,
+// not yet rounded, and every element first becomes T(acc + float(bias)), the single rounding of nn.Linear's addmm
+// (the library adds the bias to the fp32 accumulator).  bias: [(Hq + 2 Hkv) * D] in the model dtype, in qkv's column
+// order.  An item then reads 2 x 32 bytes of qkv and 2 x 16 bytes of bias; everything after is the TIN = T code.
+// 8 elements of the fp32 projection plus their bias, each rounded once to T
+template <typename T>
+__device__ __forceinline__ uint4 biased8(const float* __restrict__ src, const T* __restrict__ bias) {
+  const float4 lo = *reinterpret_cast<const float4*>(src);
+  const float4 hi = *reinterpret_cast<const float4*>(src + 4);
+  const uint4 bv = *reinterpret_cast<const uint4*>(bias);
+  const T* b = reinterpret_cast<const T*>(&bv);
+  const float acc[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+  uint4 out;
+  T* o = reinterpret_cast<T*>(&out);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j] = Elem<T>::from_f(acc[j] + Elem<T>::to_f(b[j]));
+  return out;
+}
+
+template <typename T, bool QKNORM, typename TIN = T>
 __global__ void __launch_bounds__(1024) rope_append_kernel(
-    const T* __restrict__ qkv, const T* __restrict__ cos_tab,
+    const TIN* __restrict__ qkv, const T* __restrict__ cos_tab,
     const T* __restrict__ sin_tab, const int* __restrict__ pos, const int* __restrict__ meta,
     T* __restrict__ q_out, T* __restrict__ k_cache, T* __restrict__ v_cache,
     int q_pad, int n_heads, int n_kv_heads, int D, int kv_capacity, int max_pos,
-    const T* __restrict__ q_norm_w, const T* __restrict__ k_norm_w, float eps) {
+    const T* __restrict__ q_norm_w, const T* __restrict__ k_norm_w, float eps, const T* __restrict__ bias) {
   // programmatic dependent launch: let the consumer (lade_attn_fwd) start its prologue and prefetch the cache tiles of
   // earlier steps while this grid runs; it orders itself with griddepcontrol.wait before touching what is written here
   pdl_enter();
@@ -228,9 +249,16 @@ __global__ void __launch_bounds__(1024) rope_append_kernel(
   const T* srow = sin_tab + (long long)p * D;
   for (int it = threadIdx.x; it < n_items; it += blockDim.x) {
     const int h = it / per_head, sl = it % per_head;
-    const T* src = qkv + (long long)r * ld + (long long)h * D + sl * 8;
-    uint4 a = *reinterpret_cast<const uint4*>(src);
-    uint4 b = *reinterpret_cast<const uint4*>(src + half);
+    const TIN* src = qkv + (long long)r * ld + (long long)h * D + sl * 8;
+    uint4 a, b;
+    if constexpr (std::is_same<TIN, T>::value) {
+      a = *reinterpret_cast<const uint4*>(src);
+      b = *reinterpret_cast<const uint4*>(src + half);
+    } else {
+      const T* bs = bias + (long long)h * D + sl * 8;
+      a = biased8<T>(src, bs);
+      b = biased8<T>(src + half, bs + half);
+    }
     T* dst;
     if (h < n_heads) {
       dst = q_out + ((long long)h * q_pad + r) * D + sl * 8;
@@ -410,13 +438,18 @@ static int rmsnorm_gather_impl(void* stream, const void* x, const void* delta, c
   return LADE_OK;
 }
 
-template <typename T, bool QKNORM = false>
+// TIN = float: the bias variant (qkv the fp32 projection, `bias` the fused q/k/v bias); no model has both it and QKNORM
+template <typename T, bool QKNORM = false, typename TIN = T>
 static int rope_append_impl(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab, const int32_t* pos,
                             const int32_t* meta, void* q_out, void* k_cache, void* v_cache, int32_t rows, int32_t q_pad,
                             int32_t n_heads, int32_t n_kv_heads, int32_t head_dim, int32_t kv_capacity, int32_t max_pos,
-                            const void* q_norm_w = nullptr, const void* k_norm_w = nullptr, float eps = 0.f) {
+                            const void* q_norm_w = nullptr, const void* k_norm_w = nullptr, float eps = 0.f,
+                            const void* bias = nullptr) {
+  constexpr bool BIAS = !std::is_same<TIN, T>::value;
+  static_assert(!(BIAS && QKNORM), "the bias variant has no q/k norm");
   if (!qkv || !cos_tab || !sin_tab || !pos || !meta || !q_out || !k_cache || !v_cache) return LADE_EINVAL;
   if (rows < 1 || rows > q_pad || head_dim % 16 != 0 || head_dim > 512 || n_heads < 1 || n_kv_heads < 1) return LADE_EINVAL;
+  if (BIAS && (!bias || ((uintptr_t)bias & 15) || ((uintptr_t)qkv & 15))) return LADE_EINVAL;
   if (QKNORM) {
     // a head's D/16 lanes must be an aligned group inside one warp: D/16 a power of two (D in {16, 32, ..., 512})
     if (!q_norm_w || !k_norm_w || ((uintptr_t)q_norm_w & 15) || ((uintptr_t)k_norm_w & 15)) return LADE_EINVAL;
@@ -425,10 +458,10 @@ static int rope_append_impl(void* stream, const void* qkv, const void* cos_tab, 
   // one work item (head, 8-wide slice) per thread when they fit: (32 + 2*32) heads * 8 slices = 768 threads at 7B
   int rope_threads = (((n_heads + 2 * n_kv_heads) * (head_dim / 16) + 31) / 32) * 32;
   rope_threads = rope_threads < 128 ? 128 : (rope_threads > 1024 ? 1024 : rope_threads);
-  LADE_CUDA_CHECK(launch_pdl(rope_append_kernel<T, QKNORM>, dim3(rows), dim3(rope_threads), 0, (cudaStream_t)stream,
-                             (const T*)qkv, (const T*)cos_tab, (const T*)sin_tab, (const int*)pos, (const int*)meta,
+  LADE_CUDA_CHECK(launch_pdl(rope_append_kernel<T, QKNORM, TIN>, dim3(rows), dim3(rope_threads), 0, (cudaStream_t)stream,
+                             (const TIN*)qkv, (const T*)cos_tab, (const T*)sin_tab, (const int*)pos, (const int*)meta,
                              (T*)q_out, (T*)k_cache, (T*)v_cache, q_pad, n_heads, n_kv_heads, head_dim, kv_capacity,
-                             max_pos, (const T*)q_norm_w, (const T*)k_norm_w, eps));
+                             max_pos, (const T*)q_norm_w, (const T*)k_norm_w, eps, (const T*)bias));
   return LADE_OK;
 }
 
@@ -508,6 +541,22 @@ int lade_rope_append_qknorm_f16(void* stream, const void* qkv, const void* cos_t
                                 float eps) {
   return rope_append_impl<__half, true>(stream, qkv, cos_tab, sin_tab, pos, meta, q_out, k_cache, v_cache, rows, q_pad,
                                         n_heads, n_kv_heads, head_dim, kv_capacity, max_pos, q_norm_w, k_norm_w, eps);
+}
+int lade_rope_append_bias(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab,
+                          const int32_t* pos, const int32_t* meta, void* q_out, void* k_cache, void* v_cache,
+                          int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
+                          int32_t kv_capacity, int32_t max_pos, const void* bias) {
+  return rope_append_impl<__nv_bfloat16, false, float>(stream, qkv, cos_tab, sin_tab, pos, meta, q_out, k_cache, v_cache,
+                                                       rows, q_pad, n_heads, n_kv_heads, head_dim, kv_capacity, max_pos,
+                                                       nullptr, nullptr, 0.f, bias);
+}
+int lade_rope_append_bias_f16(void* stream, const void* qkv, const void* cos_tab, const void* sin_tab,
+                              const int32_t* pos, const int32_t* meta, void* q_out, void* k_cache, void* v_cache,
+                              int32_t rows, int32_t q_pad, int32_t n_heads, int32_t n_kv_heads, int32_t head_dim,
+                              int32_t kv_capacity, int32_t max_pos, const void* bias) {
+  return rope_append_impl<__half, false, float>(stream, qkv, cos_tab, sin_tab, pos, meta, q_out, k_cache, v_cache, rows,
+                                                q_pad, n_heads, n_kv_heads, head_dim, kv_capacity, max_pos, nullptr,
+                                                nullptr, 0.f, bias);
 }
 int lade_swiglu(void* stream, const void* gate_up, void* out, int32_t rows, int32_t inter) {
   return swiglu_impl<__nv_bfloat16>(stream, gate_up, out, rows, inter);

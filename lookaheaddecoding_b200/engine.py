@@ -1,7 +1,8 @@
 """Host-side driver of the H100 lookahead/verification step.
 
 One ``LookaheadEngine`` wraps one HF ``LlamaForCausalLM`` (or ``Qwen3ForCausalLM``, whose per-head q/k RMSNorm
-runs inside ``lade_rope_append_qknorm``) on one GPU.  Per decoding step it launches
+runs inside ``lade_rope_append_qknorm``, or ``Qwen2ForCausalLM``, whose q/k/v projection biases are added to the fp32
+QKV projection inside ``lade_rope_append_bias``) on one GPU.  Per decoding step it launches
 (through the C-ABI of ``include/lade_sm100.h``):
 
     lade_step_layout -> embedding gather -> L x [ lade_rmsnorm -> QKV GEMM -> lade_rope_append ->
@@ -107,8 +108,10 @@ def decided_slots(n_emit: int, hits: Sequence[int], window_cap: int, gs: int, sa
 
 
 class LookaheadEngine:
-    """Device-resident lookahead decoding for one Llama-shaped model (batch 1, bf16 or fp16, CUDA): Llama, or Qwen3 with
-    its per-head q/k RMSNorm."""
+    """Device-resident lookahead decoding for one Llama-shaped model (batch 1, bf16 or fp16, CUDA): Llama, Qwen3 with
+    its per-head q/k RMSNorm, or Qwen2 / Qwen2.5 with biases on q_proj, k_proj and v_proj (o_proj and the MLP without).
+    On a model with those biases the QKV projection is written in fp32 and the bias is added to that accumulator before
+    the single rounding to the model dtype, as nn.Linear's addmm does."""
 
     def __init__(self, model, window_size: int, level: int, guess_set_size: int,
                  pool_from_prompt: bool = False, max_total_len: int = 4096, attn_impl: int = 0,
@@ -129,6 +132,7 @@ class LookaheadEngine:
         self.k_rmsnorm_gather = getattr(self.lib, "lade_rmsnorm_gather" + sfx)
         self.k_rope_append = getattr(self.lib, "lade_rope_append" + sfx)
         self.k_rope_append_qknorm = getattr(self.lib, "lade_rope_append_qknorm" + sfx)
+        self.k_rope_append_bias = getattr(self.lib, "lade_rope_append_bias" + sfx)
         self.k_swiglu = getattr(self.lib, "lade_swiglu" + sfx)
         self.k_argmax_rows = getattr(self.lib, "lade_argmax_rows" + sfx)
         self.k_argmax_processed = getattr(self.lib, "lade_argmax_processed" + sfx)
@@ -169,6 +173,7 @@ class LookaheadEngine:
         self.rope_theta = float(rp.get("rope_theta", getattr(cfg, "rope_theta", 10000.0)) if isinstance(rp, dict)
                                 else getattr(cfg, "rope_theta", 10000.0))
         self._check_attention_layout(model, int(max_total_len))
+        self.has_qkv_bias = self._check_biases(model)
         self.attn_impl = attn_impl
         self.use_cuda_graph = use_cuda_graph
         self.lm_cap = 1 + self.WCAP + self.G * self.GS
@@ -274,33 +279,66 @@ class LookaheadEngine:
             self.qk_eps.append(float(qn.variance_epsilon))
         self.q_norm_w, self.k_norm_w = qw, kw
 
+    def _check_biases(self, model) -> bool:
+        """True for a model whose q_proj, k_proj and v_proj carry a bias on every layer (Qwen2 / 2.5), False for one
+        without any projection bias.  Every other placement of biases is refused here, before anything is allocated:
+        the step adds biases to q, k and v only."""
+        q_norms = self.q_norm_w is not None
+        n_biased = 0
+        for li, layer in enumerate(model.model.layers):
+            a, mlp = layer.self_attn, layer.mlp
+            if getattr(a.o_proj, "bias", None) is not None:
+                raise LadeError(f"layer {li}: o_proj has a bias (Llama attention_bias=True): not supported")
+            if any(getattr(m_, "bias", None) is not None for m_ in (mlp.gate_proj, mlp.up_proj, mlp.down_proj)):
+                raise LadeError(f"layer {li}: MLP bias (mlp_bias=True) is not supported")
+            have = [getattr(getattr(a, n_), "bias", None) is not None for n_ in ("q_proj", "k_proj", "v_proj")]
+            if not any(have):
+                continue
+            if not all(have):
+                missing = [n_ for n_, h_ in zip(("q_proj", "k_proj", "v_proj"), have) if not h_]
+                raise LadeError(f"layer {li}: a bias on only some of q/k/v ({', '.join(missing)} without): not supported")
+            for n_ in ("q_proj", "k_proj", "v_proj"):
+                m_ = getattr(a, n_)
+                b = m_.bias
+                if b.dtype != self.dt or tuple(b.shape) != (m_.weight.shape[0],) or b.device != m_.weight.device:
+                    raise LadeError(f"layer {li}: {n_} bias {(tuple(b.shape), b.dtype)} is not "
+                                    f"[{m_.weight.shape[0]}] in {self.dt}: not supported")
+            if q_norms:
+                raise LadeError(f"layer {li}: q/k/v biases together with per-head q/k norms are not supported")
+            n_biased += 1
+        if 0 < n_biased < len(model.model.layers):
+            raise LadeError(f"q/k/v biases on {n_biased} of {len(model.model.layers)} layers: not supported")
+        return n_biased > 0
+
     def _fuse_weights(self):
-        """Fuse q/k/v and gate/up into single GEMM operands; re-point the HF parameters at views of
-        the fused storage so no second copy of the weights stays resident."""
+        """Fuse q/k/v and gate/up into single GEMM operands (and the q/k/v biases into one vector); re-point the HF
+        parameters at views of the fused storage so no second copy of the weights stays resident."""
         m = self.model.model
         self.embed = m.embed_tokens.weight
         self.norm_w = m.norm.weight
         self.lm_head = self.model.lm_head.weight
         self.w_qkv, self.w_o, self.w_gu, self.w_down, self.ln1, self.ln2 = [], [], [], [], [], []
+        self.b_qkv: Optional[List[torch.Tensor]] = [] if self.has_qkv_bias else None
         # a previous engine of this model already fused: reuse its storage (no second 13 GB transient) as long as
         # the HF parameters still point into it
         prev = self.model.__dict__.get("_lade_fused")
         with torch.no_grad():
             for li, layer in enumerate(m.layers):
                 a, mlp = layer.self_attn, layer.mlp
-                if any(getattr(m_, "bias", None) is not None for m_ in (a.q_proj, a.k_proj, a.v_proj, a.o_proj)):
-                    raise LadeError("attention_bias=True is not supported")
-                if any(getattr(m_, "bias", None) is not None for m_ in (mlp.gate_proj, mlp.up_proj, mlp.down_proj)):
-                    raise LadeError("mlp_bias=True is not supported")
                 nq, nk = a.q_proj.weight.shape[0], a.k_proj.weight.shape[0]
-                qkv = gu = None
+                qkv = gu = bqkv = None
                 if prev is not None and li < len(prev[0]):
                     pq, pg = prev[0][li], prev[1][li]
+                    pb = prev[2][li] if self.has_qkv_bias and len(prev) > 2 and li < len(prev[2]) else None
                     if (pq.data_ptr() == a.q_proj.weight.data_ptr() and pq[nq:].data_ptr() == a.k_proj.weight.data_ptr()
                             and pq[nq + nk:].data_ptr() == a.v_proj.weight.data_ptr()
                             and pg.data_ptr() == mlp.gate_proj.weight.data_ptr()
-                            and pg[self.I:].data_ptr() == mlp.up_proj.weight.data_ptr()):
-                        qkv, gu = pq, pg
+                            and pg[self.I:].data_ptr() == mlp.up_proj.weight.data_ptr()
+                            and (not self.has_qkv_bias or (
+                                pb is not None and pb.data_ptr() == a.q_proj.bias.data_ptr()
+                                and pb[nq:].data_ptr() == a.k_proj.bias.data_ptr()
+                                and pb[nq + nk:].data_ptr() == a.v_proj.bias.data_ptr()))):
+                        qkv, gu, bqkv = pq, pg, pb
                 if qkv is None:
                     qkv = torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], dim=0).contiguous()
                     a.q_proj.weight.data = qkv[:nq]
@@ -309,13 +347,20 @@ class LookaheadEngine:
                     gu = torch.cat([mlp.gate_proj.weight, mlp.up_proj.weight], dim=0).contiguous()
                     mlp.gate_proj.weight.data = gu[: self.I]
                     mlp.up_proj.weight.data = gu[self.I:]
+                    if self.has_qkv_bias:
+                        bqkv = torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias]).contiguous()
+                        a.q_proj.bias.data = bqkv[:nq]
+                        a.k_proj.bias.data = bqkv[nq:nq + nk]
+                        a.v_proj.bias.data = bqkv[nq + nk:]
                 self.w_qkv.append(qkv)
+                if self.has_qkv_bias:
+                    self.b_qkv.append(bqkv)
                 self.w_gu.append(gu)
                 self.w_o.append(a.o_proj.weight)
                 self.w_down.append(mlp.down_proj.weight)
                 self.ln1.append(layer.input_layernorm.weight)
                 self.ln2.append(layer.post_attention_layernorm.weight)
-        self.model.__dict__["_lade_fused"] = (self.w_qkv, self.w_gu)
+        self.model.__dict__["_lade_fused"] = (self.w_qkv, self.w_gu, self.b_qkv or [])
 
     def _rope_tables(self):
         # fp32 math then cast to the model dtype: lade/models/modeling_llama.py:240-256,:264-265
@@ -351,7 +396,10 @@ class LookaheadEngine:
         self.lp_recv = torch.zeros(self.DW * self.rec_ints, **i32)
         self.h = torch.empty(rows, self.H, dtype=bf, device=dev)
         self.xn = torch.empty(rows, self.H, dtype=bf, device=dev)
-        self.qkv = torch.empty(rows, (self.nh + 2 * self.nkv) * self.D, dtype=bf, device=dev)
+        # a model with q/k/v biases: the QKV projection's fp32 accumulator, which lade_rope_append_bias adds the bias to
+        # and rounds once
+        self.qkv = torch.empty(rows, (self.nh + 2 * self.nkv) * self.D, dtype=torch.float32 if self.has_qkv_bias else bf,
+                               device=dev)
         self.qb = torch.zeros(self.nh, rows, self.D, dtype=bf, device=dev)
         self.attn_out = torch.empty(rows, self.nh * self.D, dtype=bf, device=dev)
         self.o_buf = torch.empty(rows, self.H, dtype=bf, device=dev)
@@ -460,16 +508,22 @@ class LookaheadEngine:
         return 1
 
     def _proj(self, x, w, out) -> int:
-        """out = x @ w^T for an nn.Linear weight `w` (every projection of the step, lm_head included)."""
-        torch.mm(x, w.t(), out=out)
+        """out = x @ w^T for an nn.Linear weight `w` (every projection of the step, lm_head included).  An fp32 `out` (the
+        QKV projection of a model with q/k/v biases) receives the fp32 accumulator, not rounded to the model dtype."""
+        if out.dtype == x.dtype:
+            torch.mm(x, w.t(), out=out)
+        else:
+            torch.mm(x, w.t(), out_dtype=out.dtype, out=out)
         return 0
 
     def _rope_append(self, stream: int, l: int, qkv, qb, kc, vc, rows: int) -> int:
-        """RoPE on q and k of layer `l` (after their per-head RMSNorm on a model that has one); q to the head-major `qb`,
-        k and v appended to the layer's cache."""
+        """RoPE on q and k of layer `l` (after their per-head RMSNorm, or the q/k/v bias, on a model that has one); q to
+        the head-major `qb`, k and v appended to the layer's cache."""
         args = (stream, _ptr(qkv), _ptr(self.cos), _ptr(self.sin), _ptr(self.pos), _ptr(self.meta), _ptr(qb), _ptr(kc),
                 _ptr(vc), rows, rows, self.nh, self.nkv, self.D, self.kv_capacity, self.table_len)
-        if self.q_norm_w is None:
+        if self.b_qkv is not None:
+            check(self.k_rope_append_bias(*args, _ptr(self.b_qkv[l])), "lade_rope_append_bias")
+        elif self.q_norm_w is None:
             check(self.k_rope_append(*args), "lade_rope_append")
         else:
             check(self.k_rope_append_qknorm(*args, _ptr(self.q_norm_w[l]), _ptr(self.k_norm_w[l]), self.qk_eps[l]),
