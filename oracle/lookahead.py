@@ -292,14 +292,35 @@ def lp_window_slice(window_len: int, D: int, rank: int):
     return min(split * rank, window_len), min(split * (rank + 1), window_len)
 
 
+def step_state(step, lay, kv_len, past_tokens, fill_level, token_map, all_old, out_ids, first_guess, inp_tokens,
+               new_tokens, hits, max_hit, max_hit_idx, kv_src, kv_dst, kv_len_new, skip, n_emit, finished, filtered,
+               local) -> dict:
+    """What ``on_step`` receives after step ``step`` (1-based) has updated the loop state.
+
+    ``past_tokens``, ``token_map``, ``all_old`` and ``out_ids`` are the loop's live objects (read-only; copy what must
+    outlive the call).  ``layout`` / ``kv_len`` describe the step's rows and the committed cache before it;
+    ``inp_tokens`` are this worker's outputs on the newest window level, ``new_tokens`` the (gathered) row the window
+    took from them; ``hits`` / ``max_hit`` / ``max_hit_idx`` the decision every worker applied, and ``local`` =
+    (max_hit, max_hit_idx, hits) of this worker's own verification before the LP reduction.  ``kv_src`` (-1: no copy),
+    ``kv_dst``, ``kv_len_new`` the cache compaction, ``skip`` the tokens re-fed next step, ``n_emit`` the tokens
+    appended to ``out_ids``, ``filtered`` the newest window level after the sampling loop's EOS filter (None when
+    no filter ran) and ``finished`` the stop condition."""
+    return dict(step=step, layout=lay, kv_len=kv_len, past_tokens=past_tokens, fill_level=fill_level,
+                token_map=token_map, all_old=all_old, out_ids=out_ids, first_guess=first_guess,
+                inp_tokens=list(inp_tokens), new_tokens=list(new_tokens), hits=list(hits), max_hit=max_hit,
+                max_hit_idx=max_hit_idx, kv_src=kv_src, kv_dst=kv_dst, kv_len_new=kv_len_new, skip=skip,
+                n_emit=n_emit, finished=bool(finished), filtered=filtered, local=local)
+
+
 def greedy_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int, step_fn: StepFn,
                      compact_fn: CompactFn, pool_from_prompt: bool = False,
                      eos_token_id=None, rng: Optional[random.Random] = None,
                      trace: Optional[List[StepTrace]] = None, token_map_out: Optional[dict] = None,
-                     comm=None):
+                     comm=None, on_step: Optional[Callable[[dict], None]] = None):
     """Restatement of jacobi_greedy_search_multilevel, incl. lookahead parallelism. Returns (ids, steps).
 
     `comm` = None/LocalComm for one worker, TorchDistComm under LP (DIST_WORKERS = comm.world).
+    `on_step(state)`, if given, is called after every step's state update with the dict ``step_state`` documents.
     """
     assert N >= 3, "LEVEL must be >= 3 (past_tokens[1] must exist, decoding.py:902)"
     comm = comm or LocalComm()
@@ -356,11 +377,13 @@ def greedy_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int
             first_guess = comm.broadcast(first_guess, 0)                                 # :1024
         max_hit, max_hit_idx = 0, 0
         hits = [first_guess] + [0] * (N - 2)
+        local = (max_hit, max_hit_idx, list(hits))
         if past_tokens[1] is None:                                                       # :1038
             past_tokens[0] = past_tokens[0][1:]
             past_tokens[1] = list(inp_toks)
             if D > 1:
                 past_tokens[1] = comm.broadcast(past_tokens[1], D - 1)                   # :1045
+            new_tokens = past_tokens[1]
             fill_level += 1
         elif past_tokens[N - 2] is None:                                                 # :1049
             for level in range(fill_level + 1):
@@ -369,10 +392,12 @@ def greedy_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int
             if D > 1:
                 current = sum(comm.all_gather(current), [])                              # :1057-1058
             past_tokens[fill_level + 1] = current[1:]
+            new_tokens = current
             fill_level += 1
         else:
             if guess_tokens is not None:
                 max_hit, max_hit_idx, hits = verify_guesses(first_guess, guess_tokens, guess_res, N)
+            local = (max_hit, max_hit_idx, list(hits))
             if D > 1:                                                                    # :1088-1097
                 all_hits = comm.all_gather(max_hit)
                 max_hit = max(all_hits)
@@ -383,6 +408,7 @@ def greedy_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int
             if D > 1:
                 new_results = sum(comm.all_gather(new_results), [])                      # :1106-1107
             assert len(past_tokens[N - 2]) == W and len(new_results) == W                # :1114
+            new_tokens = new_results
             update_token_map(token_map, lst_token, past_tokens, new_results, N, W, G)    # :1116
             past_tokens[0] = past_tokens[1][1:]                                          # :1120
             for level in range(1, N - 2):
@@ -422,6 +448,10 @@ def greedy_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int
             trace.append(tr)
         out_ids = out_ids + hits[:n_emit]                                                # :1196
         first = False
+        if on_step is not None:
+            on_step(step_state(steps, lay, tr.kv_len, past_tokens, fill_level, token_map, all_old, out_ids,
+                               first_guess, inp_toks, new_tokens, hits, max_hit, max_hit_idx, tr.kv_src, kvcache_len,
+                               kv_len, guess_skip_dist, n_emit, finished, None, local))
         if finished or len(out_ids) >= max_length:                                       # :1205-1219
             break
     out_ids = out_ids[:max_length]                                                       # :1221-1225
@@ -433,12 +463,12 @@ def greedy_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int
 # --------------------------------------------------------------------------------------------
 def sample_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int, model, warper=None,
                      pool_from_prompt: bool = False, eos_token_id=None, rng: Optional[random.Random] = None,
-                     trace: Optional[list] = None):
+                     trace: Optional[list] = None, on_step: Optional[Callable[[dict], None]] = None):
     """Restatement of jacobi_sample_multilevel.  `model` provides step_fn / compact_fn / last_logits
     (oracle.llama_ref.OracleLlama); `warper(input_ids, scores)` is the HF LogitsProcessorList of
     temperature / top-k / top-p warpers.  Consumes python `random` and the global torch RNG exactly like the
     reference (random.random() per accept test :507, torch.multinomial :462,:472,:533,:545, random.choice in
-    filter_window :578-580).  Returns (ids, steps)."""
+    filter_window :578-580).  Returns (ids, steps).  `on_step` as in greedy_lookahead."""
     import torch
 
     rng = rng or random
@@ -485,6 +515,7 @@ def sample_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int
         step_len = kv_len + q
         next_token_scores = warp(input_ids_t, logits[lay.n_input - 1:lay.n_input])      # :445
         max_hit, max_hit_idx = 0, 0
+        filtered = None
         if past_tokens[1] is None:                                                       # :458-468
             probs = torch.nn.functional.softmax(next_token_scores, dim=-1)
             next_tokens = torch.multinomial(probs, num_samples=1).squeeze(1)
@@ -549,6 +580,8 @@ def sample_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int
                 for idx in range(len(past_tokens[N - 2])):
                     if past_tokens[N - 2][idx] == eos_token_id[0]:
                         past_tokens[N - 2][idx] = set_token()
+                filtered = list(past_tokens[N - 2])
+        src = -1
         if max_hit > 0:                                                                  # :583-590
             src = step_len - len(guess_tokens) + max_hit_idx * GS
             model.compact_fn(kvcache_len, src, max_hit, kvcache_len + max_hit)
@@ -575,6 +608,10 @@ def sample_lookahead(prompt: Sequence[int], max_new: int, W: int, N: int, G: int
         finished = False
         if eos_t is not None:                                                            # :636-643
             finished = bool(next_tokens.to(dev).tile(eos_t.shape[0], 1).ne(eos_t.unsqueeze(1)).prod(dim=0).max() == 0)
+        if on_step is not None:
+            on_step(step_state(steps, lay, kvcache_len - lay.n_input, past_tokens, fill_level, token_map, all_old,
+                               out_ids, hits[0], inp_toks, inp_toks, hits, max_hit, max_hit_idx, src, kvcache_len,
+                               kv_len, 0, n_emit, finished, filtered, (max_hit, max_hit_idx, list(hits))))
         if finished or len(out_ids) >= max_length:
             break
     return out_ids[:max_length], steps
