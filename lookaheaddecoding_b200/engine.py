@@ -107,6 +107,17 @@ def decided_slots(n_emit: int, hits: Sequence[int], window_cap: int, gs: int, sa
     return slots
 
 
+def attn_kv_bound(max_total_len: int, q_nonprefill: int, level: int) -> int:
+    """Upper bound of kv_len + q_len of any step an engine built for `max_total_len` runs, the surplus step
+    generate() queues before it knows the generation has ended included.  A real step starts with at most
+    max_length - 1 tokens out and emits up to N - 1 (a full accept), so the state it leaves holds at most
+    max_length + N - 2 tokens and a cache of kv_len = n_out - 1 <= max_length + N - 3 rows; any step laid out on that
+    state adds at most q_nonprefill rows.  generate() itself queues the surplus step only behind a step that starts
+    at max_length - 2 tokens out or fewer, so the steps it launches stay one row below this bound (kv_len <=
+    max_length + N - 4); the extra row keeps the bound valid for any step run on a finished state."""
+    return max_total_len + level - 3 + q_nonprefill
+
+
 class LookaheadEngine:
     """Device-resident lookahead decoding for one Llama-shaped model (batch 1, bf16 or fp16, CUDA): Llama, Qwen3 with
     its per-head q/k RMSNorm, or Qwen2 / Qwen2.5 with biases on q_proj, k_proj and v_proj (o_proj and the MLP without).
@@ -208,10 +219,12 @@ class LookaheadEngine:
         # 3 KV tiles of 128 rows per split and 8 splits per head
         self.attn_kv_bound = self.kv_capacity
         if self.attn_impl == 3:
-            self.attn_kv_bound = min(self.kv_capacity, self.max_total_len + self.q_nonprefill)
+            self.attn_kv_bound = min(self.kv_capacity, attn_kv_bound(self.max_total_len, self.q_nonprefill, self.N))
             need = -(-((self.attn_kv_bound + 127) // 128) // 3)
             if need > 8:
-                raise LadeError(f"attn_impl=3 holds at most 3072 rows of context (asked for {self.attn_kv_bound})")
+                raise LadeError(f"attn_impl=3 holds at most 3072 rows of context (asked for {self.attn_kv_bound}: "
+                                f"max_total_len {self.max_total_len} + N - 3 = {self.N - 3} rows a final accept may "
+                                f"overshoot + {self.q_nonprefill} step rows)")
             if not attn_splits:
                 self.attn_splits = max(self.attn_splits, need)
             elif self.attn_splits < need:

@@ -99,8 +99,18 @@ def additive_mask(vis: torch.Tensor, kv_len: int, dtype) -> torch.Tensor:
     return m
 
 
+# A float64 attention whose score block [H, q, kv] would exceed this many elements runs over groups of heads: the
+# result is the same per head, and a 2900-row prefill at 32 heads stays within a few GB of temporaries.
+F64_SCORE_CHUNK = 1 << 27
+
+
 def eager_attention(q, k, v, mask, n_rep: int = 1):
     """Reference eager attention numerics on [H, q, D] x [Hkv, kv, D] (modeling_llama.py:520-541)."""
+    H, R, T = q.shape[0], q.shape[1], k.shape[1]
+    if q.dtype == torch.float64 and H * R * T > F64_SCORE_CHUNK and H > n_rep:
+        hk = max(1, F64_SCORE_CHUNK // (n_rep * R * T)) * n_rep          # whole GQA groups per chunk
+        return torch.cat([eager_attention(q[h:h + hk], k[h // n_rep:(h + hk) // n_rep],
+                                          v[h // n_rep:(h + hk) // n_rep], mask, n_rep) for h in range(0, H, hk)])
     if n_rep > 1:
         k = k.repeat_interleave(n_rep, dim=0)
         v = v.repeat_interleave(n_rep, dim=0)
@@ -317,13 +327,17 @@ class OracleLlama:
     bf16 / fp16 weights give the reference's rounding points.  float64 weights give a float64 forward with no fp32
     step inside (RMSNorm statistics, softmax and logits stay float64); it needs `rope_dtype`, the precision of its
     RoPE tables: the model dtype of the 16-bit model it stands for (the device step's tables), or torch.float32
-    (HF's tables for a float64 model)."""
+    (HF's tables for a float64 model).  The embedding and lm_head of a float64 forward may stay in the model dtype:
+    the forward widens only the embedding rows it gathers, and lm_head one vocabulary chunk at a time, so a checkpoint
+    vocabulary of 152064 costs no float64 copy of either."""
+
+    LM_CHUNK = 16384            # vocabulary rows of lm_head widened at a time
 
     def __init__(self, cfg: dict, weights: Dict[str, torch.Tensor], device="cpu", rope_dtype=None):
         self.cfg = cfg
         self.dev = torch.device(device)
         self.w = {k: v.to(self.dev) for k, v in weights.items()}
-        self.dtype = self.w["lm_head.weight"].dtype
+        self.dtype = self.w["model.norm.weight"].dtype
         if self.dtype == torch.float64 and rope_dtype is None:
             raise ValueError("a float64 OracleLlama needs rope_dtype (the model dtype's tables or torch.float32)")
         self.H, self.L = cfg["hidden"], cfg["layers"]
@@ -342,22 +356,37 @@ class OracleLlama:
         self.last_hidden = None
         self.last_attn_io = None
 
+    def _qkv(self, i: int, x: torch.Tensor, q_len: int):
+        """q [nh, q_len, D], k and v [nkv, q_len, D] of layer i (the hook a model with projection biases overrides)."""
+        p = f"model.layers.{i}.self_attn."
+        return [torch.nn.functional.linear(x, self.w[p + name + "_proj.weight"]).view(q_len, heads, self.D).transpose(0, 1)
+                for name, heads in (("q", self.nh), ("k", self.nkv), ("v", self.nkv))]
+
+    def _lm_head(self, h: torch.Tensor) -> torch.Tensor:
+        lm = self.w["lm_head.weight"]
+        if lm.dtype == h.dtype:
+            return torch.nn.functional.linear(h, lm)
+        out = torch.empty(h.shape[0], lm.shape[0], dtype=h.dtype, device=h.device)
+        for c in range(0, lm.shape[0], self.LM_CHUNK):
+            out[:, c:c + self.LM_CHUNK] = h @ lm[c:c + self.LM_CHUNK].to(h.dtype).t()
+        return out
+
     # -- one forward over the step rows, returns fp32 logits [q, V] (float64 for a float64 model) ---
-    def forward_rows(self, ids, pos, vis_mask: torch.Tensor, kv_len: int, capture_layer: int = -1):
+    def forward_rows(self, ids, pos, vis_mask: torch.Tensor, kv_len: int, capture_layer: int = -1,
+                     logit_rows: Optional[List[int]] = None):
+        """`logit_rows`: the step rows whose logits are returned (in that order), default all of them."""
         w, dt = self.w, self.dtype
         ids_t = torch.as_tensor(ids, dtype=torch.long, device=self.dev)
         pos_t = torch.as_tensor(pos, dtype=torch.long, device=self.dev)
         q_len = ids_t.numel()
-        h = w["model.embed_tokens.weight"][ids_t]
+        h = w["model.embed_tokens.weight"][ids_t].to(dt)
         mask = additive_mask(vis_mask.to(self.dev), kv_len, dt)
         cos, sin = self.cos[pos_t], self.sin[pos_t]
         for i in range(self.L):
             p = f"model.layers.{i}."
             res = h
             x = rms_norm(h, w[p + "input_layernorm.weight"], self.eps)
-            q = torch.nn.functional.linear(x, w[p + "self_attn.q_proj.weight"]).view(q_len, self.nh, self.D).transpose(0, 1)
-            k = torch.nn.functional.linear(x, w[p + "self_attn.k_proj.weight"]).view(q_len, self.nkv, self.D).transpose(0, 1)
-            v = torch.nn.functional.linear(x, w[p + "self_attn.v_proj.weight"]).view(q_len, self.nkv, self.D).transpose(0, 1)
+            q, k, v = self._qkv(i, x, q_len)
             if self.qk_norm:                    # Qwen3RMSNorm over each head, before the rotary embedding
                 q = rms_norm(q, w[p + "self_attn.q_norm.weight"], self.eps)
                 k = rms_norm(k, w[p + "self_attn.k_norm.weight"], self.eps)
@@ -379,7 +408,9 @@ class OracleLlama:
             h = res + torch.nn.functional.linear(torch.nn.functional.silu(g) * u, w[p + "mlp.down_proj.weight"])
         h = rms_norm(h, w["model.norm.weight"], self.eps)
         self.last_hidden = h
-        logits = torch.nn.functional.linear(h, w["lm_head.weight"])
+        if logit_rows is not None:
+            h = h[torch.as_tensor(logit_rows, dtype=torch.long, device=self.dev)]
+        logits = self._lm_head(h)
         return logits if dt == torch.float64 else logits.float()
 
     # -- StepFn / CompactFn for oracle.lookahead.greedy_lookahead ---------------------------------

@@ -51,44 +51,6 @@ class BiasOracle(LR.OracleLlama):
             out.append(F.linear(x, self.w[p + name + ".weight"], b).view(q_len, heads, self.D).transpose(0, 1))
         return out
 
-    def forward_rows(self, ids, pos, vis_mask: torch.Tensor, kv_len: int, capture_layer: int = -1):
-        """OracleLlama.forward_rows with the biased q/k/v projections."""
-        w, dt = self.w, self.dtype
-        ids_t = torch.as_tensor(ids, dtype=torch.long, device=self.dev)
-        pos_t = torch.as_tensor(pos, dtype=torch.long, device=self.dev)
-        q_len = ids_t.numel()
-        h = w["model.embed_tokens.weight"][ids_t]
-        mask = LR.additive_mask(vis_mask.to(self.dev), kv_len, dt)
-        cos, sin = self.cos[pos_t], self.sin[pos_t]
-        for i in range(self.L):
-            p = f"model.layers.{i}."
-            res = h
-            x = LR.rms_norm(h, w[p + "input_layernorm.weight"], self.eps)
-            q, k, v = self._qkv(i, x, q_len)
-            if self.qk_norm:
-                q = LR.rms_norm(q, w[p + "self_attn.q_norm.weight"], self.eps)
-                k = LR.rms_norm(k, w[p + "self_attn.k_norm.weight"], self.eps)
-            q = (q * cos) + (LR.rotate_half(q) * sin)
-            k = (k * cos) + (LR.rotate_half(k) * sin)
-            if self.k_cache[i] is not None and kv_len > 0:
-                k = torch.cat([self.k_cache[i][:, :kv_len], k], dim=1)
-                v = torch.cat([self.v_cache[i][:, :kv_len], v], dim=1)
-            self.k_cache[i], self.v_cache[i] = k, v
-            o = LR.eager_attention(q, k, v, mask, self.nh // self.nkv)
-            if i == capture_layer:
-                self.last_attn_io = (q.clone(), k.clone(), v.clone(), o.clone())
-            o = o.transpose(0, 1).reshape(q_len, self.nh * self.D)
-            h = res + F.linear(o, w[p + "self_attn.o_proj.weight"])
-            res = h
-            x = LR.rms_norm(h, w[p + "post_attention_layernorm.weight"], self.eps)
-            g = F.linear(x, w[p + "mlp.gate_proj.weight"])
-            u = F.linear(x, w[p + "mlp.up_proj.weight"])
-            h = res + F.linear(F.silu(g) * u, w[p + "mlp.down_proj.weight"])
-        h = LR.rms_norm(h, w["model.norm.weight"], self.eps)
-        self.last_hidden = h
-        logits = F.linear(h, w["lm_head.weight"])
-        return logits if dt == torch.float64 else logits.float()
-
 
 def biased(acc: torch.Tensor, bias: torch.Tensor, dtype) -> torch.Tensor:
     """T(acc + float(bias)): acc fp32 [..., C], bias [C] in `dtype`; the sum in fp32, one rounding."""

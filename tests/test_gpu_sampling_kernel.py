@@ -10,8 +10,9 @@ is ``oracle/sampling_device.py``.
 * stream: exported uniforms == host Philox bit for bit, the offset advance, no word used twice over 200 launches,
   and the engine's steps continue one stream;
 * accept-threshold probes: uniforms 1.25 to 4 error bounds b below (must accept) or above (must reject) the float64
-  accept probability, after 0 to 4 rejections, for T in {0.05, 1, 4} with and without top-k / top-p;
-* kept set and inverse CDF of plain draws on rows built around the top-k / top-p cut-offs;
+  accept probability, after 0 to 4 rejections, for T in {0.05, 1, 4} with and without top-k / top-p, at vocabularies
+  32000, 128256 and 152064;
+* kept set and inverse CDF of plain draws on rows built around the top-k / top-p cut-offs, vocabularies to 152064;
 * the accept chain against the restatement; the distribution of the emitted (hits, max_hit_idx) against an exact
   enumeration (G-test); the EOS filter, a finished state, and run-to-run determinism.
 
@@ -262,15 +263,16 @@ def find_probes(seed, k, rejects, lo, hi, n_want, start=0, max_words=1 << 27):
     return found
 
 
-def probe_row(rng, vocab, T, p, k, spread=64):
-    """A row where position-0 candidates 0..k-1 carry 0.15 each and candidate k carries p of what remains."""
+def probe_row(rng, vocab, T, p, k, spread=64, base=100):
+    """A row where position-0 candidates 0..k-1 carry 0.15 each and candidate k carries p of what remains; the
+    candidates sit from id `base` on, the background from `base` + 100."""
     target = np.zeros(vocab)
-    cands = list(range(100, 100 + 10 * (k + 1), 10))
+    cands = list(range(base, base + 10 * (k + 1), 10))
     q = 0.15
     rest = 1.0 - q * k
     target[cands[:k]] = q
     target[cands[k]] = p * rest
-    bg = np.setdiff1d(np.arange(200, 200 + 4 * spread, 4), cands)[:spread]
+    bg = np.setdiff1d(np.arange(base + 100, base + 100 + 4 * spread, 4), cands)[:spread]
     w = np.exp(-np.linspace(0, 6, spread))
     target[bg] = max(rest * (1 - p), 1e-300) * w / w.sum()
     with np.errstate(divide="ignore"):
@@ -283,14 +285,21 @@ def probe_row(rng, vocab, T, p, k, spread=64):
 PROBE_TARGETS = [(1e-3, 0), (0.05, 1), (0.3, 3), (0.5, 4), (0.9, 2), (1 - 1e-6, 0)]
 
 
-@pytest.mark.parametrize("T,warp", [(0.05, "none"), (1.0, "none"), (4.0, "none"), (1.0, "top_k"), (0.05, "top_k"),
-                                    (4.0, "top_p")])
-def test_accept_probability_matches_float64(H, T, warp):
+# Llama-2 / CodeLlama's 32000, Llama-3's 128256 and Qwen2.5's 152064: at the larger two the candidates sit past id
+# 2^17, and every kept term of the sums (and of the top-p fixed-point mass) is visited by 100+ strides of a thread
+ACCEPT_PROBES = [(T, warp, V) for V in (32000, 128256, 152064)
+                 for T, warp in [(0.05, "none"), (1.0, "none"), (4.0, "none"), (1.0, "top_k"), (0.05, "top_k"),
+                                 (4.0, "top_p")]]
+
+
+@pytest.mark.parametrize("T,warp,vocab", ACCEPT_PROBES,
+                         ids=[f"{T}-{w}" + ("" if V == 32000 else f"-v{V}") for T, w, V in ACCEPT_PROBES])
+def test_accept_probability_matches_float64(H, T, warp, vocab):
     rng = np.random.default_rng(int(T * 100))
-    vocab, seed = 32000, 99
+    seed = 99
     checked = 0
     for p_t, k in PROBE_TARGETS:
-        lg, cands = probe_row(rng, vocab, T, p_t, k)
+        lg, cands = probe_row(rng, vocab, T, p_t, k, base=100 if vocab == 32000 else vocab - 1000)
         top_k = top_p = None
         logits = step_rows(H, lg, ld=vocab + 8)
         row = host_rows(logits, vocab)[0]
@@ -407,6 +416,14 @@ def kept_set_cases(h):
     cases.append(("exp underflows", r, 4096, 1.0, 0, 1.0))
     r = rng.normal(0, 1.0, 4096); r[:4] += 3.0; r[100:4096:2] = -100.0
     cases.append(("exp underflows, top-k 60", r, 4096, 0.5, 60, 1.0))
+    # real vocabularies past 2^17 ids (Llama-3, Qwen2.5): a flat row keeps every token under any top_p < 1 (ties are
+    # kept together), so the fixed-point top-p mass sums 152064 terms of 2^40 each
+    cases.append(("flat row, V 152064, top_p=0.5", np.full(152064, 0.75), 152064, 1.0, 0, 0.5))
+    r = rng.normal(0, 0.5, 152064); r[[3, 70000, 151000]] = [6.0, 5.5, 5.0]
+    cases.append(("top_p=0.3, V 152064", r, 152064, 1.0, 0, 0.3))
+    cases.append(("top_p=1-2^-20, V 128256", rng.normal(0, 2.0, 128256), 128256, 1.0, 0, 1 - 2.0 ** -20))
+    r = rng.normal(0, 1.0, 128256); r[[131, 127000]] += 6.0
+    cases.append(("top_k=50, T=0.7, V 128256", r, 128256, 0.7, 50, 1.0))
     return cases
 
 

@@ -209,3 +209,10 @@ def test_reference_order_attention_refuses_contexts_it_cannot_hold():
     eng = LookaheadEngine(hf, 15, 5, 15, max_total_len=1024, attn_impl=3)
     assert eng.attn_splits >= 3 and eng.attn_kv_bound <= 384 * eng.attn_splits
     eng.close()
+    # the largest capacity: 3072 rows less the 120 rows of a W15 N5 G15 step and the N - 3 = 2 rows a final full accept
+    # may leave the cache past max_length (engine.attn_kv_bound: any step laid out on that state attends to them)
+    eng = LookaheadEngine(hf, 15, 5, 15, max_total_len=2950, attn_impl=3)
+    assert eng.q_nonprefill == 120 and eng.attn_kv_bound == 3072 and eng.attn_splits == 8
+    eng.close()
+    with pytest.raises(Exception, match="attn_impl=3 holds at most 3072 rows of context"):
+        LookaheadEngine(hf, 15, 5, 15, max_total_len=2951, attn_impl=3)

@@ -173,3 +173,24 @@ def test_rope_table_choice():
     c32, _ = LR.rope_tables(128, 64, 1e4, torch.float32, "cpu")
     c64f, _ = LR.rope_tables(128, 64, 1e4, torch.float64, "cpu", table_dtype=torch.float32)
     assert torch.equal(c32.double(), c64f) and not torch.equal(c64f, c64)
+
+
+def test_memory_saving_paths_compute_the_same_forward(case, monkeypatch):
+    """What lets the float64 oracle run at checkpoint widths changes no value: the embedding and lm_head left in the
+    model dtype (only the gathered rows and one vocabulary chunk widened), logits of the asked rows only, and the
+    attention over groups of heads (whole GQA groups) when its score block is large."""
+    name, ocfg, w, ids, _ = case
+    want = oracle_logits(LR.OracleLlama(ocfg, w, rope_dtype=torch.float32), ids)
+    narrow = {k: v.to(torch.bfloat16) if k in ("model.embed_tokens.weight", "lm_head.weight") else v
+              for k, v in w.items()}
+    ref = oracle_logits(LR.OracleLlama(ocfg, {k: v.double() for k, v in narrow.items()}, rope_dtype=torch.float32), ids)
+    monkeypatch.setattr(LR.OracleLlama, "LM_CHUNK", 100)                   # several chunks, the last one partial
+    monkeypatch.setattr(LR, "F64_SCORE_CHUNK", 300)                        # one GQA group of heads at a time
+    orc = LR.OracleLlama(ocfg, narrow, rope_dtype=torch.float32)
+    assert orc.dtype == torch.float64
+    got = oracle_logits(orc, ids)
+    assert rel_err(got, ref) <= REL_TOL and rel_err(ref, want) > REL_TOL    # the narrowed weights do change the model
+    rows = [SPLIT - 1, 0, 5]
+    part = orc.forward_rows(ids[:SPLIT].tolist(), list(range(SPLIT)), torch.tril(torch.ones(SPLIT, SPLIT, dtype=torch.bool)),
+                            0, logit_rows=rows)
+    assert part.shape == (3, ocfg["vocab"]) and rel_err(part, ref[rows]) <= REL_TOL

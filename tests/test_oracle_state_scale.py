@@ -169,3 +169,66 @@ def test_admitted_edges_of_the_state_config():
             assert lib.lade_step_rows_bound(C.byref(cfg), 40, k) >= lay.q_len, (r, k)
             if r == 0:
                 assert lib.lade_step_rows_bound(C.byref(cfg), 40, k) == lay.q_len, (r, k)
+
+
+def _next_layout(s, N, G):
+    """The rows of the step after the one `s` describes (greedy_lookahead's layout code, one worker): what the step
+    generate() queues before it knows that this step ends the generation runs on."""
+    past, out = s["past_tokens"], s["out_ids"]
+    lst = s["hits"][s["max_hit"]]
+    guess = None
+    if past[N - 2] is not None and lst in s["token_map"] and G > 0:
+        guess = [t for tup in s["token_map"][lst] for t in tup] or None
+    return LA.build_step_layout(out[-1 - s["skip"]:], len(out) - 1, past, s["fill_level"], guess, N, False)
+
+
+def _launched_rows(m, prompt, max_new, W, N, G):
+    """kv_len + q_len of every step the engine's pipelined generate() launches, in order, and whether the last one
+    is the surplus step: step k + 1 is queued while step k runs unless the tokens out before step k already make step
+    k the last (engine.generate's `certainly_last`)."""
+    P, states = len(prompt), []
+
+    def on_step(s):
+        states.append(dict(rows=s["kv_len"] + s["layout"].q_len, n_out=len(s["out_ids"]), kv_new=s["kv_len_new"],
+                           nxt=_next_layout(s, N, G).q_len))
+
+    LA.greedy_lookahead(prompt, max_new, W, N, G, m.step_fn, lambda *a: None, pool_from_prompt=True,
+                        rng=random.Random(0), on_step=on_step)
+    rows = [s["rows"] for s in states]
+    n_out_before_last = states[-2]["n_out"] if len(states) > 1 else P
+    surplus = (n_out_before_last - P) + 1 < max_new
+    if surplus:
+        rows.append(states[-1]["kv_new"] + states[-1]["nxt"])
+    return rows, surplus, states[-1]["kv_new"]
+
+
+def test_reference_order_attention_bound_covers_the_surplus_step():
+    """attn_impl=3 traps when kv_len + q_len of a launched step exceeds its kv_bound.  A final multi-token accept
+    leaves the cache past max_length, and generate() has already queued one more step on that finished state: the
+    engine's bound must cover it.  Driven over every max_new_tokens of a range, on a model that accepts often."""
+    from helpers import make_lade_config
+    from lookaheaddecoding_b200 import _cabi
+    from lookaheaddecoding_b200.engine import attn_kv_bound
+    lib = _cabi.load()
+    W, N, G = 15, 5, 15
+    cfg = make_lade_config(W, N, G, 4096, 4096, pool=True)
+    q_nonprefill = max(lib.lade_step_rows_bound(C.byref(cfg), 1, k) for k in range(1, N - 1))
+    assert q_nonprefill == 120
+    # the model's own continuations are always right, and a prompt of many jumps and foreign ids fills every key's
+    # pool to G candidates: every steady step is a full accept of the full 120 rows
+    m = SS.CycleModel(4096, 5, n_ids=24, dev_per_mille=0)
+    prompt = SS.walk_prompt(m, 600, 5, jump=0.3, foreign=0.3)
+    worst_over, worst_kv, n_surplus = -10 ** 9, -10 ** 9, 0
+    for max_new in range(30, 50):
+        max_length = len(prompt) + max_new
+        rows, surplus, kv_last = _launched_rows(m, prompt, max_new, W, N, G)
+        assert max(rows) <= attn_kv_bound(max_length, q_nonprefill, N), (max_new, max(rows))
+        assert kv_last <= max_length + N - 3, max_new                     # the bound's argument
+        n_surplus += surplus
+        worst_over = max(worst_over, max(rows) - (max_length + q_nonprefill))
+        worst_kv = max(worst_kv, kv_last - max_length)
+    # a final full accept from max_length - 1 tokens out leaves kv_len = max_length + N - 3 (no step follows it in
+    # generate(), but the bound covers one); from max_length - 2 tokens out, the most that still queues the surplus
+    # step, it leaves max_length + N - 4, and the surplus step runs the full 120 rows on that: N - 4 = 1 row past
+    # the bound of max_length + q_nonprefill the engine used to pass
+    assert n_surplus > 0 and worst_kv == N - 3 and worst_over == N - 4, (n_surplus, worst_kv, worst_over)
