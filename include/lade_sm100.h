@@ -384,7 +384,9 @@ int lade_accept_update(LadeCtx* ctx, void* stream, const int32_t* argmax_slots, 
 /* Sampling verification ON DEVICE for the reference's warper set {temperature, top-k, top-p} (decoding.py:375-377;
  * top_k = 0 and top_p = 1 switch the filters off) -- replaces the host loop of
  * jacobi_sample_multilevel, lade/decoding.py:445-546 (softmax of out_logits / T :445,:485; per n-gram position the
- * accept test u < min(1, p[token]) over the n-grams still alive :495-516, zero-and-renormalise on reject :518-520,
+ * accept test over the n-grams still alive :495-516 (u <= min(1, p[token]) for the uniform u in (0, 1], which accepts
+ * with probability p like the reference's random.random() < p), zero-and-renormalise on reject :518-520 (each test
+ * normalised by the kept mass not yet rejected, summed afresh in float64: a sole survivor has p = 1),
  * residual multinomial draw :533-535; single multinomial draw on steps without candidates :458-480,:543-546) and
  * filter_window (:131-135,:578-580).  One kernel, one CTA; random numbers from a Philox4x32-10 stream whose
  * (seed, offset) live in `rng_state[2]` (device, uint64; the kernel advances the offset), so a sampling step replays

@@ -16,9 +16,17 @@
 // Here: ONE kernel, one CTA.  Row statistics (max, sum of exp) and the inverse-CDF draw are block-wide passes over the
 // vocabulary; the accept chain itself is a handful of scalar steps on thread 0.  Random numbers come from one
 // Philox4x32-10 stream (seed, offset) kept in device memory and advanced by the kernel, so the step -- forward, this
-// kernel, lade_commit_decision, KV compaction -- replays from one CUDA graph with no host round trip.  Renormalising
-// after k rejections is carried as the rejected mass: p'[t] = p[t] / (1 - sum of rejected p) (exactly what the
-// sequential divide-by-sum computes, without rewriting 32000 probabilities per rejection).
+// kernel, lade_commit_decision, KV compaction -- replays from one CUDA graph with no host round trip.
+//
+// Accept rule: curand_uniform lies in (0, 1], random.random() in [0, 1); the kernel accepts iff u <= min(1, p), which
+// accepts with probability p like the reference's r < p, so a token of probability 1 is always accepted and one of
+// probability 0 never is.
+// Renormalising after rejections: the reference divides by a fresh sum of what is left (:518-520).  The kernel
+// normalises each accept test by the kept mass not yet rejected, R: a block-wide float64 sum of the fp32 e_t over
+// the kept, not-rejected tokens, then R -= e_j per further rejection (the same fp32 e_j, so the exp errors of the
+// rejected terms cancel exactly), summed afresh whenever R falls below 2^-12 of the last fresh sum.  The block sum is
+// only run for a decision that fp32 S - rejected mass, with its error bound, cannot settle.  No 1 / (1 - rejected
+// mass) amplification: a long chain costs no accuracy, and a single survivor gets p = 1.
 #include "state.cuh"
 
 #include <curand_kernel.h>
@@ -58,6 +66,19 @@ __device__ __forceinline__ float block_reduce_sum(float v, float* s_red) {
 template <typename T>
 __device__ __forceinline__ float score_of(const T* row, int t, float temperature) {
   return Elem<T>::to_f(row[t]) / temperature;
+}
+
+__device__ __forceinline__ double block_reduce_sum_f64(double v, double* s_red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __syncthreads();
+  if (lane == 0) s_red[warp] = v;
+  __syncthreads();
+  double r = (lane < (int)(blockDim.x >> 5)) ? s_red[lane] : 0.0;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
+  return r;
 }
 
 // 16-bit float bit pattern (bf16 or fp16: sign-magnitude) -> 16-bit key that orders like the value (the logits have a
@@ -306,13 +327,29 @@ __device__ int multinomial_excluding(const T* row, int vocab, float temperature,
         for (int k = 0; k < n_z; ++k) z = z || (zset[k] == t);
         if (!z && e_of(row, t, temperature, rd) > 0.f) pick = t;
       }
-      *s_pick = pick < 0 ? 0 : pick;
+      *s_pick = pick < 0 ? 0 : pick;   // no mass outside zset: the accept chain never leaves that (see R below)
     }
     __syncthreads();
     pick = *s_pick;
   }
   __syncthreads();
   return pick;
+}
+
+// R = sum of e_t over the kept tokens not in zset[0..n_z), accumulated in float64 from the fp32 e_t (every thread
+// returns it).  Sums of positive terms only: R >= e_c for every such c, and R == e_c exactly when c is all that is left.
+template <typename T>
+__device__ double kept_mass_excluding(const T* row, int vocab, float temperature, const RowDist& rd, const int* zset,
+                                      int n_z, double* s_red) {
+  double r = 0.0;
+  for (int t = threadIdx.x; t < vocab; t += blockDim.x) {
+    const float e = e_of(row, t, temperature, rd);
+    if (e <= 0.f) continue;
+    bool z = false;
+    for (int k = 0; k < n_z && !z; ++k) z = zset[k] == t;
+    if (!z) r += (double)e;
+  }
+  return block_reduce_sum_f64(r, s_red);
 }
 
 // decision_out: the record lade_commit_decision consumes --
@@ -326,6 +363,7 @@ __device__ __forceinline__ void sample_verify_chain(int* st, const Dims& d, cons
                                                     unsigned long long* rng_state, int* __restrict__ rec, float* dbg,
                                                     float* wdbg) {
   __shared__ float s_red[32];
+  __shared__ double s_red64[32];
   __shared__ int s_cnt[256];
   __shared__ unsigned long long s_mass[256];
   __shared__ unsigned long long s_mtot[2];
@@ -334,7 +372,8 @@ __device__ __forceinline__ void sample_verify_chain(int* st, const Dims& d, cons
   __shared__ int s_pick;
   __shared__ int s_z[SMP_MAX_NGRAMS];           // tokens rejected at the current position
   __shared__ unsigned char s_alive[SMP_MAX_NGRAMS];
-  __shared__ int s_ctl[8];                      // 0 accepted?, 1 row of the next distribution, 2 n_z, 3 n_hits, 4 max_hit_idx
+  __shared__ int s_ctl[8];                      // 0 accepted?, 1 row of the next distribution, 2 n_z, 3 n_hits, 4 max_hit_idx,
+                                                // 5 R to be summed afresh
   __shared__ float s_u;
   __shared__ int s_hits[64];
 
@@ -382,31 +421,67 @@ __device__ __forceinline__ void sample_verify_chain(int* st, const Dims& d, cons
       if constexpr (WARPED) rs = row_dist_warped(row, vocab, temperature, top_k, top_p, wp, s_red, s_cnt, s_mass, s_mtot,
                                                  s_sel, wdbg);
       else rs = row_dist(row, vocab, temperature, top_k, top_p, s_red, s_cnt, s_mass, s_mtot, s_sel);
-      if (t == 0) {
-        int n_z = 0;
-        float zmass = 0.f;                      // probability mass rejected so far at this position
-        int accepted = 0;
-        for (int e = 0; e < n_ng && !accepted; ++e) {
-          if (!s_alive[e]) continue;
-          const int draft = gtok[e * GS + i];
-          bool in_z = false;
-          for (int k = 0; k < n_z; ++k) in_z = in_z || (s_z[k] == draft);
-          const float p_raw = e_of(row, draft, temperature, rs) / rs.sum;
-          const float denom = 1.f - zmass;
-          const float p = in_z ? 0.f : (denom > 0.f ? p_raw / denom : 1.f);
-          const float u = draw();
-          if (u < fminf(1.f, p)) {              // :508 (strict <)
-            accepted = 1;
-            s_hits[i] = draft;
-            s_ctl[4] = e;
-            for (int e2 = 0; e2 < n_ng; ++e2)   // :513-516 keep the n-grams that agree on this token
-              if (s_alive[e2] && gtok[e2 * GS + i] != draft) s_alive[e2] = 0;
-            s_ctl[1] = 1 + WCAP + e * GS + i;   // next distribution: the logits row after this guess token
-          } else if (!in_z) {                   // :518-520
-            s_z[n_z++] = draft;
-            zmass += p_raw;
+      // Thread 0 walks the alive n-grams.  After a rejection the fp32 S less the rejected mass brackets R to within
+      // tol (the fp32 sum's error bound, doubled; the fixed-point top-p mass is within vocab 2^-41), which settles
+      // all but the decisions whose uniform lies that close to p.  Those wait for the whole block to sum R afresh in
+      // float64; from then on R -= e_j per rejection, summed afresh again below 2^-12 of the last sum.  Between
+      // fresh sums the float64 error stays within 2^-30 of R: a sole survivor's p rounds to 1.0f, R never reaches 0.
+      int e_next = 0, n_z = 0, accepted = 0;    // thread 0's chain state
+      double rem = 0.0, ref = 0.0, zsum = 0.0;  // R once summed afresh, its last fresh value, the rejected mass
+      bool exact = false;                       // rem holds R
+      float u_held = 0.f;                       // the uniform of a decision waiting for a fresh sum
+      const double tol = (double)rs.sum * (double)((vocab + blockDim.x - 1) / blockDim.x + 12) * 0x1p-23 +
+                         (double)vocab * 0x1p-41;
+      if (t == 0) s_ctl[5] = 0;                 // 1: the block sums R afresh before thread 0 goes on
+      for (;;) {
+        if (t == 0) {
+          for (; e_next < n_ng; ++e_next) {
+            const int e = e_next;
+            if (!s_alive[e]) continue;
+            const int draft = gtok[e * GS + i];
+            bool in_z = false;
+            for (int k = 0; k < n_z && !in_z; ++k) in_z = s_z[k] == draft;
+            const float ec = in_z ? 0.f : e_of(row, draft, temperature, rs);
+            const float u = u_held > 0.f ? u_held : draw();
+            u_held = 0.f;
+            // :508 r < p on [0, 1) == u <= p on (0, 1]; p = 0 (removed by a warper, underflowed, rejected already)
+            // is never accepted
+            int verdict = 0;                    // 1 accept, -1 reject, 0 not settled yet
+            if (!(ec > 0.f)) {
+              verdict = -1;
+            } else if (n_z == 0) {
+              verdict = u <= fminf(1.f, ec / rs.sum) ? 1 : -1;
+            } else if (!exact) {
+              const double lo = (double)rs.sum - zsum - tol, hi = lo + 2.0 * tol;
+              if (lo > 0.0) {
+                if (u <= (float)fmin(1.0, (double)ec / hi)) verdict = 1;
+                else if ((float)fmin(1.0, (double)ec / lo) < u) verdict = -1;
+              }
+            } else if (rem >= 0x1p-12 * ref) {
+              verdict = u <= (float)fmin(1.0, (double)ec / rem) ? 1 : -1;
+            }
+            if (!verdict) { u_held = u; s_ctl[5] = 1; s_ctl[2] = n_z; break; }
+            if (verdict > 0) {
+              accepted = 1;
+              s_hits[i] = draft;
+              s_ctl[4] = e;
+              for (int e2 = 0; e2 < n_ng; ++e2)   // :513-516 keep the n-grams that agree on this token
+                if (s_alive[e2] && gtok[e2 * GS + i] != draft) s_alive[e2] = 0;
+              s_ctl[1] = 1 + WCAP + e * GS + i;   // next distribution: the logits row after this guess token
+              break;
+            } else if (!in_z) {                 // :518-520
+              s_z[n_z++] = draft;
+              rem -= (double)ec;
+              zsum += (double)ec;
+            }
           }
         }
+        __syncthreads();
+        if (!s_ctl[5]) break;
+        const double r = kept_mass_excluding(row, vocab, temperature, rs, s_z, s_ctl[2], s_red64);
+        if (t == 0) { rem = ref = r; exact = true; s_ctl[5] = 0; }
+      }
+      if (t == 0) {
         s_ctl[0] = accepted;
         s_ctl[2] = n_z;
         if (accepted) s_ctl[3] = i + 1;

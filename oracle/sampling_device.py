@@ -67,7 +67,7 @@ def verify_given_uniforms(out_row: np.ndarray, guess_rows: Optional[np.ndarray],
             p = min(1.0, float(probs_next[draft]))                                         # :505
             u = next(it); used += 1
             checks.append(("accept", u, p, draft))
-            if u < p:                                                                      # :508
+            if u <= p:                                    # :508 r < p for r in [0, 1) == u <= p for u in (0, 1]
                 hits.append(draft)
                 max_hit_idx = e
                 alive = [g for g in alive if guess_tokens[g * gs + i] == draft]            # :513-516

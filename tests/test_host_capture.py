@@ -73,7 +73,7 @@ def _winners_from_checks(want, guess, gs):
             n += 1
             _, u, p, draft = checks[k]
             k += 1
-            if u < p:
+            if u <= p:
                 break
         else:
             return winners                               # a draw ended the chain

@@ -67,7 +67,7 @@ def verify_given_uniforms(out_row: np.ndarray, guess_rows: Optional[np.ndarray],
             p = min(1.0, float(probs_next[draft]))
             u = next(it); used += 1
             checks.append(("accept", u, p, draft))
-            if u < p:
+            if u <= p:                                   # the kernel's rule on (0, 1]: sampling_device.py
                 hits.append(draft)
                 max_hit_idx = e
                 alive = [g for g in alive if guess_tokens[g * gs + i] == draft]
